@@ -70,7 +70,7 @@ int vq_ctx_create(int device, VqContext** out_ctx) {
     if (cudaMalloc(&c->spd_counter, 2 * VQ_SPD_SLOTS * sizeof(uint32_t)) != cudaSuccess) { delete c; vq_set_error("cudaMalloc failed"); return VQ_ERR_OUT_OF_MEMORY; }
     cudaMemset(c->spd_counter, 0, 2 * VQ_SPD_SLOTS * sizeof(uint32_t));
     {   // persisting-L2 carve-out for K1's sampling copies (vq_forward.cu), OPT-IN (VQ_L2_PERSIST=1): the set-aside takes L2 away
-        // from the 531 MB that stream through per 4K frame, and 102 MB of copies do not fit a 50 MB L2 anyway. The device limit is
+        // from the 531 MB that stream through per 4K frame, and 68 MB of copies do not fit a 50 MB L2 anyway. The device limit is
         // process-wide state.
         const char* e = getenv("VQ_L2_PERSIST");
         int maxPersist = 0, maxWindow = 0;

@@ -6,8 +6,9 @@
 //   mbarrier ring in shared memory, the result leaves as one STG.128 per pixel; one thread shades TWO pixels (two
 //   independent dependency chains through the light loop); the light array is staged once per
 //   CTA into shared memory; the IBL cubemaps and the BRDF LUT are gathered from L2-resident sampling copies
-//   (pair / footprint records, 102 MB at the reference sizes) with five 32-byte record loads per pixel, because the
-//   L1 data pipe — one wavefront per distinct line of a divergent gather — is what bounds this kernel (DESIGN.md §4).
+//   (bordered texels / footprint records, 68 MB at the reference sizes) with five 32-byte gathers per pixel, each read by
+//   two neighbouring lanes together (see "lane-pair record gathers"), because the L1 data pipe — one wavefront per distinct
+//   line of a divergent gather — is what bounds this kernel (DESIGN.md §4).
 // The math is PSMain's with per-pixel invariants hoisted out of the light loops (N, V, N.V, the
 // Smith-G term of V, F0, kD factors). Discontinuities are evaluated exactly as the oracle does:
 //   * `D < l.range` uses an unfused |L-P|^2 and a per-light threshold on the squared distance that is
@@ -28,13 +29,16 @@ namespace {
 
 // Sampling copy of a cubemap. Every face of every mip is a (N+2)x(N+2) grid of bordered texel positions, the 1-texel
 // border holding the neighbouring faces' edge texels (corners: the mean of the three texels that meet there), so
-// that the seamless bilinear footprint never leaves the face. Each position (i,j) stores the PAIR {t(i,j), t(i+1,j)}
-// as one 32-byte record: a bilinear footprint is two records, each one 32-byte sector, instead of four scattered texels.
+// that the seamless bilinear footprint never leaves the face. One float4 per position: a bilinear footprint is two rows of two
+// adjacent texels, {t(i,j), t(i+1,j)} and {t(i,j+1), t(i+1,j+1)}, 32 contiguous bytes each, instead of four scattered texels.
 // A gather whose lanes go to unrelated texels costs one L1 wavefront per distinct 128-byte line it touches, so the number
-// of distinct lines per pixel is what the layout minimises. mipOffset[] are record offsets of face 0 per mip.
+// of distinct lines per pixel is what the layout and the loads minimise: lanes 2q and 2q+1 read each other's footprint rows
+// together (cube_issue / ldg_pair), the even lane t(i) and the odd lane t(i+1), so one instruction touches at most 16 places
+// (a row crosses a line boundary once in 8 positions). mipOffset[] are position offsets of face 0 per mip.
 struct CubeV { const float4* p; int res, mips; uint32_t mipOffset[16]; };
 // Footprint copy of the BRDF LUT: record (cx,cy), cx = clamp(x0+1, 0, W), holds the CLAMP-addressed 2x2 footprint
-// {p(x0,y0), p(x0+1,y0), p(x0,y0+1), p(x0+1,y0+1)} as 4 x float2 = 32 bytes: one record (one sector) per pixel.
+// {p(x0,y0), p(x0+1,y0), p(x0,y0+1), p(x0+1,y0+1)} as 4 x float2 = 32 bytes: one record (one sector) per pixel, half .a the
+// row y0 and half .b the row y0+1, read by a lane pair like a row of a cube footprint.
 struct LutV { const float4* q; int w, h; };
 struct F8 { float4 a, b; };
 
@@ -141,25 +145,11 @@ __device__ float4 bordered_texel(const float4* __restrict__ src, int res, int mi
     return make_float4((a.x + b.x + c.x) * (1.0f / 3.0f), (a.y + b.y + c.y) * (1.0f / 3.0f),
                        (a.z + b.z + c.z) * (1.0f / 3.0f), (a.w + b.w + c.w) * (1.0f / 3.0f));
 }
-// packed cube (mip-major / face-minor, N x N faces) -> sampling copy: one {t(i,j), t(i+1,j)} record per bordered position
-// (the last position of a row repeats itself; it is never the left tap of a footprint)
+// packed cube (mip-major / face-minor, N x N faces) -> sampling copy: one texel per bordered position
 __global__ void __launch_bounds__(256) cube_pad_kernel(const float4* __restrict__ src, float4* __restrict__ dst,
                                                         int res, int mips, uint32_t totalPadded) {
-    for (uint32_t idx = blockIdx.x * 256u + threadIdx.x; idx < totalPadded; idx += gridDim.x * 256u) {
-        // is idx the last position of its row?  rows are (N+2) long and faces/mips are whole rows, so walk the mips
-        uint32_t rem = idx; int P = res + 2;
-        for (int m = 0; m < mips; ++m) {
-            P = (res >> m) + 2;
-            const uint32_t sz = 6u * (uint32_t)P * (uint32_t)P;
-            if (rem < sz) break;
-            rem -= sz;
-        }
-        const bool last = (rem % (uint32_t)P) == (uint32_t)(P - 1);
-        const float4 v0 = bordered_texel(src, res, mips, idx);
-        const float4 v1 = last ? v0 : bordered_texel(src, res, mips, idx + 1u);
-        dst[2 * (size_t)idx] = v0;
-        dst[2 * (size_t)idx + 1] = v1;
-    }
+    for (uint32_t idx = blockIdx.x * 256u + threadIdx.x; idx < totalPadded; idx += gridDim.x * 256u)
+        dst[idx] = bordered_texel(src, res, mips, idx);
 }
 
 // BRDF LUT (float2, pitched) -> footprint records (see LutV): (W+1) x (H+1) records of 32 bytes
@@ -463,17 +453,17 @@ static_assert(FWD_AHEAD >= 1 && FWD_AHEAD < FWD_STAGES, "the lookahead must leav
 struct FaceRec { uint32_t base; uint32_t P; float halfN; float c0; };     // first record of the face, row stride, N/2, N/2 - 0.5
 static_assert(sizeof(FaceRec) == 16, "one LDS.128");
 
-// L1 policy of a gather: 0 = allocate, 1 = L1::no_allocate, 2 = L1::evict_last
+// L1 policy of a gather: 0 = allocate, 1 = L1::no_allocate, 2 = L1::evict_last. A lane pair reads its two pixels' footprints
+// in consecutive instructions, and neighbouring pixels' footprints often share lines, so every gather allocates in L1.
 #ifndef FWD_L1_DIFF
 #define FWD_L1_DIFF 0
 #endif
 #ifndef FWD_L1_SPEC
-#define FWD_L1_SPEC 1
+#define FWD_L1_SPEC 0
 #endif
 #ifndef FWD_L1_LUT
-#define FWD_L1_LUT 1
+#define FWD_L1_LUT 0
 #endif
-// one 32-byte record as two 128-bit loads from the same sector (sm_90 has no 256-bit LDG)
 template <int POLICY>
 __device__ __forceinline__ float4 ldg128(const float4* p) {
     float4 r;
@@ -485,48 +475,93 @@ __device__ __forceinline__ float4 ldg128(const float4* p) {
         asm("ld.global.nc.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(r.x), "=f"(r.y), "=f"(r.z), "=f"(r.w) : "l"(p));
     return r;
 }
-template <int POLICY>
-__device__ __forceinline__ F8 ldg_rec(const float4* p) {            // 32-byte aligned record, read-only path
-    F8 r; r.a = ldg128<POLICY>(p); r.b = ldg128<POLICY>(p + 1); return r;
+// ---- lane-pair record gathers ----
+// A record here is the 32 bytes one bilinear row needs: two adjacent cube texels, or a LUT footprint (one sector). sm_90 has no
+// 256-bit load, so a record takes two LDG.128. If every lane read its own record with both, each instruction would touch up to 32
+// unrelated lines and every line would be paid for twice. So lanes 2q and 2q+1 read their two records TOGETHER: in one
+// instruction both read the even lane's record (the even lane its half .a, the odd lane its half .b), in the other both read the
+// odd lane's record (the even lane .b, the odd lane .a). Each instruction touches at most 16 places and each lane still issues
+// two loads per record. Every lane then holds the .a half of its own record and the .b half of its partner's, and one shuffle
+// per component swaps the .b halves. Every lane of the warp takes part (pixels off a ragged row are aliased, never masked off),
+// so the shuffles use the full mask.
+__device__ __forceinline__ bool odd_lane() { return (threadIdx.x & 1u) != 0u; }
+// record k starts at float4 index STRIDE*k: STRIDE 1 for a cube (record = texel k and its right neighbour), 2 for the LUT.
+// iE, iO: float4 indices of what this lane reads of the even lane's record (.a on an even lane, .b on an odd one) and of the odd
+// lane's record (.b on an even lane, .a on an odd one), given this lane's record `rec`
+template <uint32_t STRIDE>
+__device__ __forceinline__ void pair_halves(uint32_t rec, uint32_t& iE, uint32_t& iO) {
+    const uint32_t mine = STRIDE * rec;
+    const uint32_t other = __shfl_xor_sync(0xffffffffu, mine, 1) + 1u;          // the partner's record, second half
+    const bool odd = odd_lane();
+    iE = odd ? other : mine; iO = odd ? mine : other;
 }
-struct CubeLoad { F8 r0, r1; float fx, fy; };                     // rows j0 and j0+1: {t(i0), t(i0+1)} each
-// A gather is split into "issue" (address + the record loads) and "finish" (the lerps) so that the loads of several
-// gathers are in flight before the first one is consumed.
-// maxRec: last record a footprint may start at (clamps the address for NaN/inf directions: no surface => no normal)
+struct HalfPair { float4 e, o; };          // what this lane read of the even lane's record and of the odd lane's record
 template <int POLICY>
-__device__ __forceinline__ CubeLoad cube_issue(const float4* __restrict__ recs, FaceRec f, uint32_t maxRec, float sx, float sy) {
+__device__ __forceinline__ HalfPair ldg_pair(const float4* __restrict__ base, uint32_t iE, uint32_t iO) {
+    HalfPair h; h.e = ldg128<POLICY>(base + iE); h.o = ldg128<POLICY>(base + iO); return h;
+}
+// this lane's own record: its .a half is the one this lane read, its .b half comes from the partner. Only the first N components
+// of each half are exchanged (a cube blend reads rgb); the rest are zero.
+template <int N>
+__device__ __forceinline__ F8 own_record(const HalfPair& h) {
+    const bool odd = odd_lane();
+    const float he[4] = {h.e.x, h.e.y, h.e.z, h.e.w}, ho[4] = {h.o.x, h.o.y, h.o.z, h.o.w};
+    float a[4] = {0.0f, 0.0f, 0.0f, 0.0f}, b[4] = {0.0f, 0.0f, 0.0f, 0.0f};
+#pragma unroll
+    for (int k = 0; k < N; ++k) {
+        a[k] = odd ? ho[k] : he[k];
+        b[k] = __shfl_xor_sync(0xffffffffu, odd ? he[k] : ho[k], 1);        // send the partner's .b, receive our own
+    }
+    F8 rec; rec.a = make_float4(a[0], a[1], a[2], a[3]); rec.b = make_float4(b[0], b[1], b[2], b[3]);
+    return rec;
+}
+
+struct CubeLoad { HalfPair r0, r1; float fx, fy; };               // rows j0 and j0+1: {t(i0), t(i0+1)} each
+// A gather is split into "issue" (addresses + the loads) and "finish" (the exchange and the lerps) so that the loads of several
+// gathers are in flight before the first one is consumed.
+// maxRec: last position a footprint may start at (clamps the address for NaN/inf directions: no surface => no normal)
+// UNIFORM_P: the row stride f.P is the same for every lane (the diffuse cube has one mip), so only the first row's offset is exchanged
+template <int POLICY, bool UNIFORM_P>
+__device__ __forceinline__ CubeLoad cube_issue(const float4* __restrict__ texels, FaceRec f, uint32_t maxRec, float sx, float sy) {
     const float x = fmaf(sx, f.halfN, f.c0), y = fmaf(-sy, f.halfN, f.c0);       // texel space: (s*0.5+0.5)*N - 0.5
     const float xf = floorf(x), yf = floorf(y);                                  // in [-1, N-1] for every finite direction
     CubeLoad L;
     L.fx = x - xf; L.fy = y - yf;
     const uint32_t off = min(f.base + (uint32_t)((int)yf + 1) * f.P + (uint32_t)((int)xf + 1), maxRec);
-    const float4* p = recs + 2u * off;
-    L.r0 = ldg_rec<POLICY>(p); L.r1 = ldg_rec<POLICY>(p + 2u * f.P);
+    uint32_t e0, o0, e1, o1;
+    pair_halves<1u>(off, e0, o0);
+    if (UNIFORM_P) { e1 = e0 + f.P; o1 = o0 + f.P; }
+    else pair_halves<1u>(off + f.P, e1, o1);
+    L.r0 = ldg_pair<POLICY>(texels, e0, o0); L.r1 = ldg_pair<POLICY>(texels, e1, o1);
     return L;
 }
 // bilinear blend of the footprint as pairs {x,y}, {z,w} of one pixel
 __device__ __forceinline__ float3 cube_finish(const CubeLoad& L) {
+    const F8 q0 = own_record<3>(L.r0), q1 = own_record<3>(L.r1);
     const f2 fx = bc(L.fx), fy = bc(L.fy);
-    const f2 a0 = mk(L.r0.a.x, L.r0.a.y), a1 = mk(L.r0.a.z, L.r0.a.w), b0 = mk(L.r0.b.x, L.r0.b.y), b1 = mk(L.r0.b.z, L.r0.b.w);
-    const f2 c0 = mk(L.r1.a.x, L.r1.a.y), c1 = mk(L.r1.a.z, L.r1.a.w), d0 = mk(L.r1.b.x, L.r1.b.y), d1 = mk(L.r1.b.z, L.r1.b.w);
+    const f2 a0 = mk(q0.a.x, q0.a.y), a1 = mk(q0.a.z, q0.a.w), b0 = mk(q0.b.x, q0.b.y), b1 = mk(q0.b.z, q0.b.w);
+    const f2 c0 = mk(q1.a.x, q1.a.y), c1 = mk(q1.a.z, q1.a.w), d0 = mk(q1.b.x, q1.b.y), d1 = mk(q1.b.z, q1.b.w);
     const f2 t0 = fma2(fx, b0 - a0, a0), t1 = fma2(fx, b1 - a1, a1);
     const f2 u0 = fma2(fx, d0 - c0, c0), u1 = fma2(fx, d1 - c1, c1);
     const f2 r0 = fma2(fy, u0 - t0, t0), r1 = fma2(fy, u1 - t1, t1);
     return f3(r0.v.x, r0.v.y, r1.v.x);
 }
-struct LutLoad { F8 q; float fx, fy; };
+struct LutLoad { HalfPair q; float fx, fy; };
 __device__ __forceinline__ LutLoad lut_issue(const LutV& l, float u, float v) {   // bilinear, CLAMP
     const float x = fmaf(u, (float)l.w, -0.5f), y = fmaf(v, (float)l.h, -0.5f);
     const float x0 = floorf(x), y0 = floorf(y);
     LutLoad L;
     L.fx = x - x0; L.fy = y - y0;
     const int cx = min(max((int)x0 + 1, 0), l.w), cy = min(max((int)y0 + 1, 0), l.h);
-    L.q = ldg_rec<FWD_L1_LUT>(l.q + 2u * (uint32_t)(cy * (l.w + 1) + cx));
+    uint32_t e, o;
+    pair_halves<2u>((uint32_t)(cy * (l.w + 1) + cx), e, o);
+    L.q = ldg_pair<FWD_L1_LUT>(l.q, e, o);
     return L;
 }
 __device__ __forceinline__ float2 lut_finish(const LutLoad& L) {    // record = {p00, p10 | p01, p11} as float2 each
+    const F8 q = own_record<4>(L.q);
     const f2 fx = bc(L.fx), fy = bc(L.fy);
-    const f2 p00 = mk(L.q.a.x, L.q.a.y), p10 = mk(L.q.a.z, L.q.a.w), p01 = mk(L.q.b.x, L.q.b.y), p11 = mk(L.q.b.z, L.q.b.w);
+    const f2 p00 = mk(q.a.x, q.a.y), p10 = mk(q.a.z, q.a.w), p01 = mk(q.b.x, q.b.y), p11 = mk(q.b.z, q.b.w);
     const f2 t = fma2(fx, p10 - p00, p00), u = fma2(fx, p11 - p01, p01);
     return fma2(fy, u - t, t).v;
 }
@@ -550,13 +585,13 @@ __device__ __forceinline__ void env_issue(EnvLoads& E, const FwdParams& P, const
     int face; float sx, sy;
     dir_to_face(Nr, face, sx, sy);
     FaceRec fd; fd.P = (uint32_t)P.diff.res + 2u; fd.base = (uint32_t)face * fd.P * fd.P; fd.halfN = P.diffHalfN; fd.c0 = P.diffHalfN - 0.5f;
-    E.D = cube_issue<FWD_L1_DIFF>(P.diff.p, fd, P.diffMaxRec, sx, sy);
+    E.D = cube_issue<FWD_L1_DIFF, true>(P.diff.p, fd, P.diffMaxRec, sx, sy);
     if (SPEC) {
         const float3 R0 = reflect(-V, Ns);
         const float3 R = ROT ? f3(R0.x * P.cosB - R0.z * P.sinB, R0.y, R0.x * P.sinB + R0.z * P.cosB) : R0;
         dir_to_face(R, face, sx, sy);
         const int mip = min(max((int)(roughness * (float)P.maxLod), 0), P.spec.mips - 1);
-        E.S = cube_issue<FWD_L1_SPEC>(P.spec.p, sFace[face * 16 + mip], P.specMaxRec, sx, sy);
+        E.S = cube_issue<FWD_L1_SPEC, false>(P.spec.p, sFace[face * 16 + mip], P.specMaxRec, sx, sy);
         E.L = lut_issue(P.lut, nsnv, roughness);                                 // (saturate(dot(s.N, V)), roughness)
     }
 }
@@ -778,14 +813,15 @@ uint64_t padded_texels(int res, int mips) {
     for (int m = 0; m < mips; ++m) { const uint64_t p = (uint64_t)(res >> m) + 2; n += 6 * p * p; }
     return n;
 }
-// bytes of a sampling copy: the records plus one mip-0 row of slack, so that a footprint whose first record was clamped to
-// the last record (a non-finite direction: pixels without a surface carry a zero normal) still reads inside the allocation
-size_t padded_bytes(int res, int mips) { return (size_t)(padded_texels(res, mips) + (uint64_t)res + 3u) * 32u; }
+// bytes of a sampling copy: the texels plus one mip-0 row and a texel of slack, so that a footprint whose first position was
+// clamped to the last position (a non-finite direction: pixels without a surface carry a zero normal) still reads inside the
+// allocation
+size_t padded_bytes(int res, int mips) { return (size_t)(padded_texels(res, mips) + (uint64_t)res + 3u) * 16u; }
 bool cube_desc_ok(const VqCubemap& c) {
     return c.ptr && c.res >= 1 && c.mips >= 1 && c.mips <= 16 && (c.res >> (c.mips - 1)) >= 1 &&
            padded_texels(c.res, c.mips) < (1ull << 30);
 }
-// builds the sampling copy of `c` into `dst` (padded_texels() records of 32 bytes) on `stream`
+// builds the sampling copy of `c` into `dst` (padded_texels() texels of 16 bytes) on `stream`
 int pad_cube(const VqCubemap& c, float4* dst, cudaStream_t stream) {
     const uint32_t total = (uint32_t)padded_texels(c.res, c.mips);
     unsigned blocks = (total + 255u) / 256u;
