@@ -126,48 +126,42 @@ def _sky_setup(hw=256, hh=128, smooth=True):
     return pyr, levels
 
 
-@pytest.mark.parametrize("w,h,yaw,pitch", [(96, 54, 0.0, 0.0), (257, 33, 1.3, -0.4), (64, 64, -2.6, 0.9), (1, 1, 0.5, 0.1)])
-def test_skydome_matches_oracle(ctx, vq, orc, w, h, yaw, pitch):
+@pytest.mark.parametrize("w,h,yaw,pitch,rows,masked", [
+    pytest.param(96, 54, 0.0, 0.0, None, False, id="96-54-0.0-0.0"),
+    pytest.param(257, 33, 1.3, -0.4, None, False, id="257-33-1.3--0.4"),
+    pytest.param(64, 64, -2.6, 0.9, None, False, id="64-64--2.6-0.9"),
+    pytest.param(1, 1, 0.5, 0.1, None, False, id="1-1-0.5-0.1"),
+    # the kernel shades rows y, y+1 of a column per thread: a ragged width with an odd row count, a row range that starts on an
+    # odd row under a mask, a single row, a 3840-wide band
+    pytest.param(257, 33, -0.9, 0.3, None, False, id="pairs-257x33"),
+    pytest.param(160, 91, -0.9, 0.3, (7, 60), True, id="pairs-160x91-rows7-60-masked"),
+    pytest.param(64, 1, -0.9, 0.3, None, False, id="pairs-64x1"),
+    pytest.param(3840, 17, -0.9, 0.3, (2, 17), False, id="pairs-3840x17-rows2-17")])
+def test_skydome_matches_oracle(ctx, vq, orc, w, h, yaw, pitch, rows, masked):
+    """strict bound on the smooth HDRI; outside the row range and where the mask has a surface the base image stays as it was"""
     from vqengine_b200 import synth
     hw, hh = 256, 128
     pyr, levels = _sky_setup(hw, hh)
     _, inv = synth.sky_view_proj(yaw, pitch, 1.1, w / h)
     inv32 = inv.astype(np.float32).reshape(16)
-    ref = orc.skydome(pyr, hw, hh, levels, inv32, np.zeros((h, w, 4), dtype=np.float32))
-    dpyr = dev(pyr)
-    out = torch.zeros((h, w, 4), dtype=torch.float32, device="cuda")
-    ctx.skydome(inv32, vq.pyramid_of(dpyr, hw, hh, levels), out)
-    r = assert_abs(f"skydome{w}x{h}", host(out), ref)
-    print(r)
-
-
-@pytest.mark.parametrize("w,h,rows,masked", [(257, 33, None, False), (160, 91, (7, 60), True), (64, 1, None, False), (3840, 17, (2, 17), False)])
-def test_skydome_pair_kernel_equals_single_pixel_kernel(ctx, vq, orc, w, h, rows, masked, monkeypatch):
-    """two pixels per thread (the default) against one pixel per thread: the same operations per pixel, so the frames agree
-    to rounding noise of the rsqrt seeds at most; odd row counts, a row range starting on an odd row, a mask"""
-    from vqengine_b200 import synth
-    hw, hh = 512, 256
-    pyr, levels = _sky_setup(hw, hh, smooth=False)
-    _, inv = synth.sky_view_proj(-0.9, 0.3, 1.0, w / h)
-    inv32 = inv.astype(np.float32).reshape(16)
     rng = np.random.default_rng(3)
-    mask = rng.random((h, w, 4), dtype=np.float32) + 0.1
-    mask[rng.random((h, w)) < 0.5, :3] = 0.0
     base = rng.random((h, w, 4), dtype=np.float32)
-    dpyr = dev(pyr)
-
-    def run():
-        out = dev(base)
-        kw = {"normal_mask": dev(mask)} if masked else {}
-        if rows: kw.update(row_begin=rows[0], row_end=rows[1])
-        ctx.skydome(inv32, vq.pyramid_of(dpyr, hw, hh, levels), out, **kw)
-        return host(out)
-
-    pair = run()
-    monkeypatch.setenv("VQ_SKYDOME_PAIR", "0")
-    single = run()
-    assert np.array_equal(pair == base, single == base)                   # the same pixels written
-    assert np.abs(pair - single).max() <= 1e-5 * max(1.0, float(np.abs(single).max()))
+    mask = None
+    if masked:
+        mask = rng.random((h, w, 4), dtype=np.float32) + 0.1
+        mask[rng.random((h, w)) < 0.5, :3] = 0.0
+    ref = orc.skydome(pyr, hw, hh, levels, inv32, base.copy(), normal_mask=mask, rows=rows)
+    out = dev(base)
+    kw = {"normal_mask": dev(mask)} if masked else {}
+    if rows: kw.update(row_begin=rows[0], row_end=rows[1])
+    ctx.skydome(inv32, vq.pyramid_of(dev(pyr), hw, hh, levels), out, **kw)
+    got = host(out)
+    r = assert_abs(f"skydome{w}x{h}", got, ref)
+    print(r)
+    untouched = np.zeros((h, w), dtype=bool)
+    if masked: untouched |= (mask[..., :3] != 0.0).any(axis=2)
+    if rows: untouched[:rows[0]] = True; untouched[rows[1]:] = True
+    assert np.array_equal(got[untouched], base[untouched])
 
 
 def test_skydome_noisy_hdri_mask_and_rows(ctx, vq, orc):

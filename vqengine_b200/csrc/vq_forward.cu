@@ -20,10 +20,6 @@
 
 using namespace vq;
 
-#ifndef FWD_BACKOFF
-#define FWD_BACKOFF 128        // ns the producer thread sleeps between polls of an empty[] barrier (0: spin)
-#endif
-
 namespace {
 
 
@@ -194,10 +190,7 @@ struct Acc2 { f2 ax, ay, az, bx, by, bz, cx, cy, cz; };   // sum over lights of 
 // N.H with the oracle's exact operation sequence (correctly rounded div/sqrt, no FMA contraction): V, Wo,
 // N, Wi, H as BRDF.hlsl:166-169 / Lighting.hlsl:312 write them. T_EXACT = 0.02 bounds the fast path's
 // relative error in D by 2*dt/t <= 2*5e-7/0.02 = 5e-5; the slow path runs for < 1 % of pixel-light pairs.
-#ifndef FWD_T_EXACT
-#define FWD_T_EXACT 0.02f
-#endif
-constexpr float T_EXACT = FWD_T_EXACT;
+constexpr float T_EXACT = 0.02f;
 
 // dot_u, sqrt_rn_inrange, rcp_rn_prepare / div_rn_inrange, len2_inrange: vq_common.cuh (shared with the PCF kernel)
 // v / sqrt(dot(v,v)) with correctly rounded sqrt and divisions (== the oracle's normalize)
@@ -333,11 +326,7 @@ __device__ __forceinline__ void shade_all_lights(const Px2& s, Acc2& acc, const 
     const int numPoint = P.numPoint, numSpot = P.numSpot;
     // ---- point lights, then point casters (Lighting.hlsl:308-322; PSMain :310-313,321-340):
     //      in range <=> d2 < d2Limit (== length(Lw-P) < l.range, exactly) ----
-#ifndef FWD_LIGHT_UNROLL
-#define FWD_LIGHT_UNROLL 1      // 2: two lights interleaved (more ILP for the dependent MUFU/FMA chains, ~20 more registers)
-#endif
-    constexpr int kLightUnroll = FWD_LIGHT_UNROLL;
-#pragma unroll kLightUnroll
+#pragma unroll 1
     for (int i = 0; i < numPoint; ++i) {
         const SPoint l = P.pts[i];                                       // constant bank, warp-uniform index
         const LightVec2 L = light_vector2(s, l.pos);
@@ -397,15 +386,14 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
                      : "=r"(done) : "r"(bar), "r"(parity) : "memory");
     } while (!done);
 }
-__device__ __forceinline__ void mbar_wait_backoff(uint32_t bar, uint32_t parity) {   // single-thread waits: do not steal issue slots
+// single-thread waits (the producer on an empty[] barrier): 128 ns of sleep between polls, so as not to steal issue slots
+__device__ __forceinline__ void mbar_wait_backoff(uint32_t bar, uint32_t parity) {
     uint32_t done;
     for (;;) {
         asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}"
                      : "=r"(done) : "r"(bar), "r"(parity) : "memory");
         if (done) break;
-#if FWD_BACKOFF
-        __nanosleep(FWD_BACKOFF);
-#endif
+        __nanosleep(128);
     }
 }
 __device__ __forceinline__ uint64_t l2_evict_first_policy() {
@@ -435,16 +423,10 @@ __device__ __forceinline__ void st_stream_hint(float4* p, float4 v, uint64_t pol
 // copy per plane for the tile FWD_AHEAD iterations ahead (full[] mbarriers count the bytes), every thread reads
 // ITS texels back with LDS when it needs them and releases the stage (empty[] mbarriers) when its pixels are
 // stored. Nothing of the G-buffer is live in registers across the light loop: albedo/metalness/ao, the raw
-// normal and the emissive texel are (re-)read from the stage after it.
-#ifndef FWD_STAGES
-#define FWD_STAGES 2           // shared-memory stages
-#endif
-#ifndef FWD_AHEAD
-#define FWD_AHEAD 1            // tiles requested ahead of the one being shaded (< FWD_STAGES)
-#endif
-#ifndef FWD_CTAS_PER_SM
-#define FWD_CTAS_PER_SM 4
-#endif
+// normal and the emissive texel are (re-)read from the stage after it. 3 CTAs per SM measured 8 % slower (DESIGN.md §9).
+constexpr int FWD_STAGES = 2;          // shared-memory stages
+constexpr int FWD_AHEAD = 1;           // tiles requested ahead of the one being shaded (< FWD_STAGES)
+constexpr int FWD_CTAS_PER_SM = 4;
 static_assert(FWD_AHEAD >= 1 && FWD_AHEAD < FWD_STAGES, "the lookahead must leave at least one stage for the tile being shaded");
 
 // ---- environment taps -----------------------------------------------------------------------------------
@@ -453,26 +435,11 @@ static_assert(FWD_AHEAD >= 1 && FWD_AHEAD < FWD_STAGES, "the lookahead must leav
 struct FaceRec { uint32_t base; uint32_t P; float halfN; float c0; };     // first record of the face, row stride, N/2, N/2 - 0.5
 static_assert(sizeof(FaceRec) == 16, "one LDS.128");
 
-// L1 policy of a gather: 0 = allocate, 1 = L1::no_allocate, 2 = L1::evict_last. A lane pair reads its two pixels' footprints
-// in consecutive instructions, and neighbouring pixels' footprints often share lines, so every gather allocates in L1.
-#ifndef FWD_L1_DIFF
-#define FWD_L1_DIFF 0
-#endif
-#ifndef FWD_L1_SPEC
-#define FWD_L1_SPEC 0
-#endif
-#ifndef FWD_L1_LUT
-#define FWD_L1_LUT 0
-#endif
-template <int POLICY>
+// Every gather allocates in L1: a lane pair reads its two pixels' footprints in consecutive instructions, and neighbouring
+// pixels' footprints often share lines (L1::no_allocate measured 3-12 % slower, DESIGN.md §9).
 __device__ __forceinline__ float4 ldg128(const float4* p) {
     float4 r;
-    if (POLICY == 1)
-        asm("ld.global.nc.L1::no_allocate.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(r.x), "=f"(r.y), "=f"(r.z), "=f"(r.w) : "l"(p));
-    else if (POLICY == 2)
-        asm("ld.global.nc.L1::evict_last.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(r.x), "=f"(r.y), "=f"(r.z), "=f"(r.w) : "l"(p));
-    else
-        asm("ld.global.nc.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(r.x), "=f"(r.y), "=f"(r.z), "=f"(r.w) : "l"(p));
+    asm("ld.global.nc.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(r.x), "=f"(r.y), "=f"(r.z), "=f"(r.w) : "l"(p));
     return r;
 }
 // ---- lane-pair record gathers ----
@@ -496,9 +463,8 @@ __device__ __forceinline__ void pair_halves(uint32_t rec, uint32_t& iE, uint32_t
     iE = odd ? other : mine; iO = odd ? mine : other;
 }
 struct HalfPair { float4 e, o; };          // what this lane read of the even lane's record and of the odd lane's record
-template <int POLICY>
 __device__ __forceinline__ HalfPair ldg_pair(const float4* __restrict__ base, uint32_t iE, uint32_t iO) {
-    HalfPair h; h.e = ldg128<POLICY>(base + iE); h.o = ldg128<POLICY>(base + iO); return h;
+    HalfPair h; h.e = ldg128(base + iE); h.o = ldg128(base + iO); return h;
 }
 // this lane's own record: its .a half is the one this lane read, its .b half comes from the partner. Only the first N components
 // of each half are exchanged (a cube blend reads rgb); the rest are zero.
@@ -521,7 +487,7 @@ struct CubeLoad { HalfPair r0, r1; float fx, fy; };               // rows j0 and
 // gathers are in flight before the first one is consumed.
 // maxRec: last position a footprint may start at (clamps the address for NaN/inf directions: no surface => no normal)
 // UNIFORM_P: the row stride f.P is the same for every lane (the diffuse cube has one mip), so only the first row's offset is exchanged
-template <int POLICY, bool UNIFORM_P>
+template <bool UNIFORM_P>
 __device__ __forceinline__ CubeLoad cube_issue(const float4* __restrict__ texels, FaceRec f, uint32_t maxRec, float sx, float sy) {
     const float x = fmaf(sx, f.halfN, f.c0), y = fmaf(-sy, f.halfN, f.c0);       // texel space: (s*0.5+0.5)*N - 0.5
     const float xf = floorf(x), yf = floorf(y);                                  // in [-1, N-1] for every finite direction
@@ -532,7 +498,7 @@ __device__ __forceinline__ CubeLoad cube_issue(const float4* __restrict__ texels
     pair_halves<1u>(off, e0, o0);
     if (UNIFORM_P) { e1 = e0 + f.P; o1 = o0 + f.P; }
     else pair_halves<1u>(off + f.P, e1, o1);
-    L.r0 = ldg_pair<POLICY>(texels, e0, o0); L.r1 = ldg_pair<POLICY>(texels, e1, o1);
+    L.r0 = ldg_pair(texels, e0, o0); L.r1 = ldg_pair(texels, e1, o1);
     return L;
 }
 // bilinear blend of the footprint as pairs {x,y}, {z,w} of one pixel
@@ -555,7 +521,7 @@ __device__ __forceinline__ LutLoad lut_issue(const LutV& l, float u, float v) { 
     const int cx = min(max((int)x0 + 1, 0), l.w), cy = min(max((int)y0 + 1, 0), l.h);
     uint32_t e, o;
     pair_halves<2u>((uint32_t)(cy * (l.w + 1) + cx), e, o);
-    L.q = ldg_pair<FWD_L1_LUT>(l.q, e, o);
+    L.q = ldg_pair(l.q, e, o);
     return L;
 }
 __device__ __forceinline__ float2 lut_finish(const LutLoad& L) {    // record = {p00, p10 | p01, p11} as float2 each
@@ -566,18 +532,11 @@ __device__ __forceinline__ float2 lut_finish(const LutLoad& L) {    // record = 
     return fma2(fy, u - t, t).v;
 }
 
-// the environment lookups and the final composition of ONE pixel (PSMain :290-293, Lighting.hlsl:360-395, BRDF.hlsl:177-207)
-//   texel : shared-memory address of the pixel's position texel,  V/nsnv : normalize(cam-P), saturate(dot(s.N, V))
-//   la/lb/lc : the light sums  sum w*col*{(1-fc), fc*spec, spec}
-//   Ns : the surface normal as normalize(Ns)*|Ns| (within an ulp of the raw texel; it only steers the two cube lookups)
 // The environment lookups of one pixel, split into "issue" (the five record gathers: diffuse cube x2, specular cube x2, LUT, with
-// their bilinear weights) and "compose" (the blends + the final composition), so that the kernel can put BOTH pixels' gathers in
-// flight before it consumes either (FWD_JOINT_ISSUE): a thread then waits for the L2/HBM latency once per pair instead of once per
-// pixel.
+// their bilinear weights) and "compose" (the blends + the final composition), so that the kernel puts BOTH pixels' gathers in
+// flight before it consumes either: a thread then waits for the L2/HBM latency once per pair instead of once per pixel.
+//   V/nsnv : normalize(cam-P), saturate(dot(s.N, V))
 //   Ns : the surface normal as normalize(Ns)*|Ns| (within an ulp of the raw texel; it only steers the two cube lookups)
-#ifndef FWD_JOINT_ISSUE
-#define FWD_JOINT_ISSUE 1
-#endif
 struct EnvLoads { CubeLoad D, S; LutLoad L; };
 template <bool ROT, bool SPEC>
 __device__ __forceinline__ void env_issue(EnvLoads& E, const FwdParams& P, const FaceRec* __restrict__ sFace, float3 V, float nsnv, float3 Ns, float roughness) {
@@ -585,13 +544,13 @@ __device__ __forceinline__ void env_issue(EnvLoads& E, const FwdParams& P, const
     int face; float sx, sy;
     dir_to_face(Nr, face, sx, sy);
     FaceRec fd; fd.P = (uint32_t)P.diff.res + 2u; fd.base = (uint32_t)face * fd.P * fd.P; fd.halfN = P.diffHalfN; fd.c0 = P.diffHalfN - 0.5f;
-    E.D = cube_issue<FWD_L1_DIFF, true>(P.diff.p, fd, P.diffMaxRec, sx, sy);
+    E.D = cube_issue<true>(P.diff.p, fd, P.diffMaxRec, sx, sy);
     if (SPEC) {
         const float3 R0 = reflect(-V, Ns);
         const float3 R = ROT ? f3(R0.x * P.cosB - R0.z * P.sinB, R0.y, R0.x * P.sinB + R0.z * P.cosB) : R0;
         dir_to_face(R, face, sx, sy);
         const int mip = min(max((int)(roughness * (float)P.maxLod), 0), P.spec.mips - 1);
-        E.S = cube_issue<FWD_L1_SPEC, false>(P.spec.p, sFace[face * 16 + mip], P.specMaxRec, sx, sy);
+        E.S = cube_issue<false>(P.spec.p, sFace[face * 16 + mip], P.specMaxRec, sx, sy);
         E.L = lut_issue(P.lut, nsnv, roughness);                                 // (saturate(dot(s.N, V)), roughness)
     }
 }
@@ -647,18 +606,13 @@ __device__ __forceinline__ void finish_pair(const FwdParams& P, const FaceRec* _
     const f2 Nrx = s.Nx * s.nsLen, Nry = s.Ny * s.nsLen, Nrz = s.Nz * s.nsLen;
     EnvLoads eA, eB;
     env_issue<ROT, SPEC>(eA, P, sFace, f3(s.Vx.v.x, s.Vy.v.x, s.Vz.v.x), nsnv.v.x, f3(Nrx.v.x, Nry.v.x, Nrz.v.x), roughness.v.x);
-#if FWD_JOINT_ISSUE
     env_issue<ROT, SPEC>(eB, P, sFace, f3(s.Vx.v.y, s.Vy.v.y, s.Vz.v.y), nsnv.v.y, f3(Nrx.v.y, Nry.v.y, Nrz.v.y), roughness.v.y);
-#endif
     const float4 oA = compose_pixel<SPEC>(P, s.texA, nsnv.v.x, roughness.v.x, ao.v.x, f3(acc.ax.v.x, acc.ay.v.x, acc.az.v.x),
                                           f3(acc.bx.v.x, acc.by.v.x, acc.bz.v.x), f3(acc.cx.v.x, acc.cy.v.x, acc.cz.v.x), eA);
     if (validA) {   // one STG.128 per destination; peer destinations are mapped NVLink addresses (fused compute + gather)
         if (MULTI) { for (int q = 0; q < P.nOut; ++q) st_stream(P.outs[q].row(P.dstRowOffset + y) + xA, oA); }
         else st_stream_hint(P.outs[0].row(P.dstRowOffset + y) + xA, oA, l2_evict_first_policy());
     }
-#if !FWD_JOINT_ISSUE
-    env_issue<ROT, SPEC>(eB, P, sFace, f3(s.Vx.v.y, s.Vy.v.y, s.Vz.v.y), nsnv.v.y, f3(Nrx.v.y, Nry.v.y, Nrz.v.y), roughness.v.y);
-#endif
     const float4 oB = compose_pixel<SPEC>(P, s.texB, nsnv.v.y, roughness.v.y, ao.v.y, f3(acc.ax.v.y, acc.ay.v.y, acc.az.v.y),
                                           f3(acc.bx.v.y, acc.by.v.y, acc.bz.v.y), f3(acc.cx.v.y, acc.cy.v.y, acc.cz.v.y), eB);
     if (validB) {
@@ -1017,28 +971,10 @@ int vq_forward_launch_multi(VqContext* ctx, const VqPerFrameData* pf, const VqPe
         VQ_CUDA_OK(cudaFuncSetAttribute(forward_kernel<false, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
         attrSet.store(true, std::memory_order_release);
     }
-    // Experiment kept behind VQ_L2_PERSIST=1 (off by default, see vq_context.cu): a PERSISTING access-policy window over the one
-    // allocation that holds the sampling copies, as a per-launch attribute (the caller's stream state is not touched). Without it
-    // the G-buffer streams through with evict_first and the copies compete with it for L2.
-    cudaLaunchAttribute attr[1];
-    unsigned nAttr = 0;
-    if (prepared && ctx->l2_persist_bytes > 0 && ctx->env_used_bytes > 0) {
-        cudaAccessPolicyWindow w;
-        w.base_ptr = ctx->env_all;
-        w.num_bytes = ctx->env_used_bytes < (size_t)ctx->l2_window_max ? ctx->env_used_bytes : (size_t)ctx->l2_window_max;
-        const double ratio = (double)ctx->l2_persist_bytes / (double)w.num_bytes;
-        w.hitRatio = ratio >= 1.0 ? 1.0f : (float)ratio;
-        w.hitProp = cudaAccessPropertyPersisting;
-        w.missProp = cudaAccessPropertyStreaming;
-        attr[0].id = cudaLaunchAttributeAccessPolicyWindow;
-        attr[0].val.accessPolicyWindow = w;
-        nAttr = 1;
-    }
     auto launch = [&](auto kernel) -> int {
         cudaLaunchConfig_t cfg;
         memset(&cfg, 0, sizeof(cfg));
         cfg.gridDim = dim3(gx, gy); cfg.blockDim = dim3(FWD_THREADS); cfg.dynamicSmemBytes = smem; cfg.stream = stream;
-        cfg.attrs = attr; cfg.numAttrs = nAttr;
         VQ_CUDA_OK(cudaLaunchKernelEx(&cfg, kernel, P));
         return VQ_OK;
     };
@@ -1096,14 +1032,13 @@ extern "C" int vq_environment_prepare(VqContext* ctx, const VqEnvironmentMaps* e
     const bool hasSpec = env->irradiance_specular.ptr != nullptr, hasLut = env->brdf_lut.ptr != nullptr;
     if (hasSpec) VQ_REQUIRE(cube_desc_ok(env->irradiance_specular), "bad cubemap descriptor (irradiance_specular)");
     if (hasLut) VQ_REQUIRE(vq_image_ok(env->brdf_lut, 8) && env->brdf_lut.width <= 8192 && env->brdf_lut.height <= 8192, "bad BRDF LUT descriptor");
-    // ONE allocation for the three sampling copies (diffuse | specular | LUT footprints, 256-byte aligned parts): the forward
-    // kernel can then put a single L2 access-policy window over all of its L2-resident side data
+    // ONE allocation for the three sampling copies (diffuse | specular | LUT footprints, 256-byte aligned parts): one buffer
+    // to grow and free instead of three
     auto up = [](size_t b) { return (b + 255) & ~(size_t)255; };
     const size_t bD = up(padded_bytes(env->irradiance_diffuse.res, env->irradiance_diffuse.mips));
     const size_t bS = hasSpec ? up(padded_bytes(env->irradiance_specular.res, env->irradiance_specular.mips)) : 0;
     const size_t bL = hasLut ? up(lut_footprint_bytes(env->brdf_lut)) : 0;
     rc = ensure_bytes(&ctx->env_all, &ctx->env_all_bytes, bD + bS + bL); if (rc) return rc;
-    ctx->env_used_bytes = bD + bS + bL;
     ctx->env_diff = ctx->env_all;
     ctx->env_spec = hasSpec ? (char*)ctx->env_all + bD : nullptr;
     ctx->env_lut = hasLut ? (char*)ctx->env_all + bD + bS : nullptr;

@@ -3,11 +3,6 @@
 // (upload | shade | download) so that PCIe traffic in both directions overlaps the kernel; with pinned
 // host memory (cudaHostRegister / cudaMallocHost) the copies are truly asynchronous.
 #include "vq_common.cuh"
-#include <stdlib.h>
-
-namespace {
-constexpr int kMaxChunks = 16;
-}
 
 extern "C" int vq_forward_lighting_host(VqContext* ctx, const VqPerFrameData* pf, const VqPerViewLightingData* pv,
                                         const VqGBuffer* hgb, const VqEnvironmentMaps* denv, VqImage hout) {
@@ -46,8 +41,8 @@ extern "C" int vq_forward_lighting_host(VqContext* ctx, const VqPerFrameData* pf
     dgb.emissive = hasEm ? VqImage{base + 4 * planeBytes, W, H, rowBytes} : VqImage{nullptr, 0, 0, 0};
 
     // chunks pipelined over the copy-in / compute / copy-out streams; 8 at 4K keeps both link directions busy with few launches
-    int chunks = H >= 256 ? 8 : (H >= 16 ? 4 : 1);
-    if (const char* e = getenv("VQ_HOST_CHUNKS")) { const int c = atoi(e); if (c >= 1 && c <= kMaxChunks && c <= H) chunks = c; }   // tuning knob
+    // (two events per chunk: at most 16 of the context's 32)
+    const int chunks = H >= 256 ? 8 : (H >= 16 ? 4 : 1);
     const int rowsPer = (H + chunks - 1) / chunks;
     cudaStream_t sUp = ctx->streams[0], sRun = ctx->streams[1], sDown = ctx->streams[2];
     const VqImage* hp[4] = {&hgb->position_ao, &hgb->normal_roughness, &hgb->albedo_metalness, &hgb->emissive};
