@@ -376,6 +376,10 @@ void orc_sample_cube(const float* cube, int res, int mips, const float d[3], int
     const float4 r = SampleCubeLevel(Cubemap{cube, res, mips}, make3(d[0], d[1], d[2]), mip);
     out[0] = r.x; out[1] = r.y; out[2] = r.z; out[3] = r.w;
 }
+// the same over n directions (dirs: n x 3, out: n x 4), one mip each (mips: n ints)
+void orc_sample_cube_n(const float* cube, int res, int mips, const float* dirs, const int* mip, int64_t n, float* out) {
+    for (int64_t k = 0; k < n; ++k) orc_sample_cube(cube, res, mips, dirs + 3 * k, mip[k], out + 4 * k);
+}
 void orc_sample_equirect(const float* pyr, int w, int h, int levels, float u, float v, float lod, float out[4]) {
     const float4 r = SampleEquirectLevel(Pyramid{pyr, w, h, levels}, make2(u, v), lod);
     out[0] = r.x; out[1] = r.y; out[2] = r.z; out[3] = r.w;
@@ -468,6 +472,9 @@ void orc_apply_reflections(float* scene, const float* reflection, const float* b
 // ---- probes used by the compiled-shader pin (tests/test_hlsl_ref.py; oracle/ref_shim/hlsl_ref_shim.cpp) ------------
 void orc_sample_lut(const float* lut, int w, int h, float u, float v, float out[2]) {
     const float2 r = SampleLUT(Image{lut, w, h, (size_t)w * 2, 2}, u, v); out[0] = r.x; out[1] = r.y;
+}
+void orc_sample_lut_n(const float* lut, int w, int h, const float* uv, int64_t n, float* out) {
+    for (int64_t k = 0; k < n; ++k) orc_sample_lut(lut, w, h, uv[2 * k], uv[2 * k + 1], out + 2 * k);
 }
 float orc_sample_point2d(const float* map, int w, int h, float u, float v) { return SamplePoint2D(map, w, h, u, v); }
 float orc_sample_point_cube(const float* cube, int res, const float d[3]) { return SamplePointCube(cube, res, make3(d[0], d[1], d[2])); }

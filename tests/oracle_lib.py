@@ -81,6 +81,24 @@ def forward_lighting(pf, pv, planes, diff_cube, diff_res, spec_cube, spec_res, s
     return out
 
 
+def sample_cube(cube, res, mips, dirs, mip) -> np.ndarray:
+    """SampleCubeLevel over n directions: dirs (n, 3), mip an int or (n,) ints -> (n, 4)"""
+    d = _f(dirs).reshape(-1, 3)
+    m = np.ascontiguousarray(np.broadcast_to(np.asarray(mip, dtype=np.int32), (d.shape[0],)))
+    out = np.zeros((d.shape[0], 4), np.float32)
+    lib().orc_sample_cube_n(_p(_f(cube)), res, mips, _p(d), m.ctypes.data_as(C.POINTER(C.c_int)), C.c_int64(d.shape[0]), _p(out))
+    return out
+
+
+def sample_lut(lut, u, v) -> np.ndarray:
+    """SampleLUT (bilinear CLAMP) of a [H, W, 2] LUT at n coordinates -> (n, 2)"""
+    l = _f(lut)
+    uv = _f(np.stack(np.broadcast_arrays(np.asarray(u, np.float32).ravel(), np.asarray(v, np.float32).ravel()), axis=1))
+    out = np.zeros((uv.shape[0], 2), np.float32)
+    lib().orc_sample_lut_n(_p(l), l.shape[1], l.shape[0], _p(uv), C.c_int64(uv.shape[0]), _p(out))
+    return out
+
+
 def hdri_build_mips(level0: np.ndarray, levels: int) -> np.ndarray:
     h, w = level0.shape[:2]
     n = int(lib().orc_pyramid_texel_count(w, h, levels))
