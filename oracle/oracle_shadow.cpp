@@ -22,11 +22,17 @@ namespace orc {
 namespace {
 inline float3 f3(const VqFloat3& v) { return {v.x, v.y, v.z}; }
 inline int wrap(int i, int n) { const int r = i % n; return r < 0 ? r + n : r; }
+// float -> int as D3D converts (NaN -> 0, saturated): the C++ conversion of NaN is undefined; a NaN coordinate comes from a
+// light-space position with x = z = w = 0, whose depth comparisons are all false whichever texel it reads
+inline int floor_to_int(float x) {
+    const float f = std::floor(x);
+    return f != f ? 0 : (f >= 2147483648.0f ? 2147483647 : (f < -2147483648.0f ? (-2147483647 - 1) : (int)f));
+}
 }  // namespace
 
 // Texture2D(Array).Sample(PointSampler, uv).x on one slice
 float SamplePoint2D(const float* map, int w, int h, float u, float v) {
-    const int x = wrap((int)std::floor(u * (float)w), w), y = wrap((int)std::floor(v * (float)h), h);
+    const int x = wrap(floor_to_int(u * (float)w), w), y = wrap(floor_to_int(v * (float)h), h);
     return map[(size_t)y * w + x];
 }
 // TextureCubeArray.Sample(PointSampler, float4(dir, index)).x on one cube ([face][y][x])
@@ -34,8 +40,8 @@ float SamplePointCube(const float* cube, int res, float3 dir) {
     int face; float sx, sy;
     DirectionToCubeFace(dir, &face, &sx, &sy);                       // ndc coordinates in [-1,1], y up
     const float s = sx * 0.5f + 0.5f, t = -sy * 0.5f + 0.5f;
-    const int x = std::min(std::max((int)std::floor(s * (float)res), 0), res - 1);
-    const int y = std::min(std::max((int)std::floor(t * (float)res), 0), res - 1);
+    const int x = std::min(std::max(floor_to_int(s * (float)res), 0), res - 1);
+    const int y = std::min(std::max(floor_to_int(t * (float)res), 0), res - 1);
     return cube[((size_t)face * res + y) * res + x];
 }
 

@@ -28,6 +28,19 @@ void hostcheck_pcf_records(const VqPerFrameData* pf, const VqPerViewLightingData
         out[i] = vqshadow::pcf_record(L, ld(pos), ld(nrm));
     }
 }
+// the same tap counts handed to an array instead of the record: [n_pixels][11], -1 where a slot is not reported
+void hostcheck_pcf_counts(const VqPerFrameData* pf, const VqPerViewLightingData* pv, const VqShadowMaps* sm,
+                          const float* pos, const float* nrm, int n_pixels, int* out) {
+    vqshadow::ShadowLights L;
+    vqshadow::fill_shadow_lights(L, *pf, *pv, *sm);
+    for (int i = 0; i < n_pixels; ++i) {
+        auto ld = [&](const float* p) { return vqshadow::v3(vqshadow::F(p[4 * i]), vqshadow::F(p[4 * i + 1]), vqshadow::F(p[4 * i + 2])); };
+        vqshadow::ArraySink c;
+        for (int k = 0; k < 11; ++k) c.c[k] = -1;
+        vqshadow::caster_counts(L, ld(pos), ld(nrm), c);
+        for (int k = 0; k < 11; ++k) out[11 * i + k] = c.c[k];
+    }
+}
 void hostcheck_per_frame_without_casters(const VqPerFrameData* pf, VqPerFrameData* out) { *out = vqshadow::per_frame_without_casters(*pf); }
 
 // the launcher's sequence (vq_depth_min_pyramid) with the kernels' texel function run in loops
