@@ -240,6 +240,9 @@ VQ_API int vq_gaussian_blur_y(VqContext* ctx, const VqBlurParams* params, VqImag
 
 /* ------------------------------------------------------------------------------------------
  * K6  Tonemapper.  Replaces the dispatch at SceneRendering.cpp:2640-2656 + CSMain (Tonemapper.hlsl:110-151).
+ *     Domain limit of the sRGB curve: Reinhard c / (c + 1) divides with the fast reciprocal, so a channel whose finite
+ *     c + 1 exceeds 2^126 in magnitude gives 0 (the shader's division gives 1). Inputs up to 2^126, which include the
+ *     engine's whole RGBA16F range, match the shader to 1e-4; Inf and NaN give NaN as in the shader.
  * ------------------------------------------------------------------------------------------ */
 VQ_API int vq_tonemap(VqContext* ctx, const VqTonemapperParams* params, VqImage in, VqImage out, void* stream);
 
@@ -255,6 +258,14 @@ VQ_API int vq_cas(VqContext* ctx, const uint32_t cas_const[8], VqImage in, VqIma
  * K8  FSR1 EASU.  Replaces SceneRendering.cpp:2711-2734 + FSR_EASU_CSMain (AMDFidelityFX.hlsl:247-288)
  *     -> FsrEasuF (FSR1.0/ffx_fsr1.h:315-437). easu_const = FFSR1_EASU::EASUConstantBlock (16 words).
  *     Gathers use the engine's sampler addressing: VQ_ADDRESS_WRAP (RootSignatures.cpp:525) by default.
+ *     con0 must have been built for these images (vq_fsr_easu_con with viewport <= input size, output = out's size).
+ *     Before launching, the call evaluates the kernels' own texel positions floor(o * con0.xy + con0.zw) at the first and
+ *     last output pixel of each axis (they bound all others) and returns VQ_ERR_INVALID_ARG, with nothing launched, when
+ *       - any con0 value is not finite;
+ *       - a tap (texels -1 .. +2 around those positions) leaves [-W, 2W) x [-H, 2H), W = max(in.width, 3),
+ *         H = max(in.height, 3) (the range the WRAP fold handles), e.g. constants left over from before a resize;
+ *       - on the upscaling path (0 < con0.x, con0.y <= 1) a 32 x 8 output tile would need more than 32 x 8 input texels.
+ *     Every constant vq_fsr_easu_con builds for viewport <= input <= 8192 and output <= 16384 passes.
  * ------------------------------------------------------------------------------------------ */
 enum { VQ_ADDRESS_WRAP = 0, VQ_ADDRESS_CLAMP = 1 };
 VQ_API int vq_fsr_easu(VqContext* ctx, const uint32_t easu_const[16], int address_mode,

@@ -6,6 +6,7 @@
 // served by L1 (3x3 / 12-tap stencils). Math follows the HLSL the engine ships (file:line cited per
 // kernel); parity against oracle/ is tested in tests/test_post_gpu.py.
 #include "vq_common.cuh"
+#include "vq_easu_check.cuh"
 
 using namespace vq;
 
@@ -736,11 +737,16 @@ extern "C" int vq_fsr_easu(VqContext* ctx, const uint32_t con[16], int address_m
     VQ_REQUIRE(address_mode == VQ_ADDRESS_WRAP || address_mode == VQ_ADDRESS_CLAMP, "easu: unknown address mode");
     VQ_REQUIRE(in.ptr != out.ptr, "easu: in-place is not supported");
     EasuCon c; memcpy(&c, con, 16);
+    const float c0[4] = {c.c0x, c.c0y, c.c0z, c.c0w};
+    const vqeasu::Verdict v = vqeasu::check(c0, in.width, in.height, out.width, out.height);
+    VQ_REQUIRE(v != vqeasu::EASU_NONFINITE, "easu: con0 is not finite");
+    VQ_REQUIRE(v != vqeasu::EASU_TAPS_OUTSIDE, "easu: con0 puts taps outside [-w, 2w) x [-h, 2h) of the input (constants not built for these images?)");
+    VQ_REQUIRE(v != vqeasu::EASU_TILE_FOOTPRINT, "easu: con0 needs more than 32x8 input texels per 32x8 output tile");
     cudaStream_t st = (cudaStream_t)stream;
-    // ratio <= 1 (upscale or 1:1) and the footprint of a 32x16 output tile fits the staged tile: shared-memory path
-    const bool up = c.c0x > 0.0f && c.c0y > 0.0f && c.c0x <= 1.0f && c.c0y <= 1.0f;
-    // exact 2x (FsrEasuCon(w, h, w, h, 2w, 2h)): one thread per input texel, a 2x2 output quad each
-    const bool x2 = c.c0x == 0.5f && c.c0y == 0.5f && c.c0z == -0.25f && c.c0w == -0.25f && out.width == 2 * in.width && out.height == 2 * in.height;
+    // exact 2x (FsrEasuCon(w, h, w, h, 2w, 2h)): one thread per input texel, a 2x2 output quad each;
+    // ratio <= 1 (upscale or 1:1): the input footprint of a 32x8 output tile is staged in shared memory
+    const vqeasu::Path path = vqeasu::path(c0, in.width, in.height, out.width, out.height);
+    const bool x2 = path == vqeasu::EASU_2X, up = path == vqeasu::EASU_UP;
     if (x2) {
         // 'f' texels k = -1 .. W-1, m = -1 .. H-1
         const dim3 grid((in.width + 1 + E2_BX - 1) / E2_BX, (in.height + 1 + E2_BY - 1) / E2_BY);
