@@ -175,6 +175,9 @@ VQ_API int vq_environment_invalidate(VqContext* ctx);
 /* ------------------------------------------------------------------------------------------
  * K11 HDRI mip pyramid, 2x2 MIN filter, alpha = 1.  Replaces VQ_DXGI_UTILS::MipImage
  *     (DXGIUtils.cpp:289-317) called from TextureManager.cpp:714-727. Level 0 must be filled.
+ *     MIN is the reference's std::min(a, b) = (b < a) ? b : a, nested min(s0, min(s1, min(s2, s3))) over the block's
+ *     (0,0), (1,0), (0,1), (1,1) texels, for any float input: a NaN survives only in s0, a +0 / -0 tie keeps the earlier
+ *     operand. Level sizes are floor-halved; an odd last row / column is not read.
  * ------------------------------------------------------------------------------------------ */
 VQ_API int vq_hdri_build_mips(VqContext* ctx, VqPyramid hdri, void* stream);
 

@@ -7,12 +7,12 @@ namespace {
 
 struct PyrV { const float4* p; int w, h, levels; uint32_t off[16]; };
 
-PyrV make_pyr(const VqPyramid& hd) {
+inline PyrV make_pyr(const VqPyramid& hd) {
     PyrV v; v.p = (const float4*)hd.ptr; v.w = hd.width; v.h = hd.height; v.levels = hd.levels;
     for (int l = 0; l < 16; ++l) v.off[l] = l < hd.levels ? (uint32_t)vq_pyramid_offset(hd.width, hd.height, l) : 0u;
     return v;
 }
-bool pyr_ok(const VqPyramid& hd) {
+inline bool pyr_ok(const VqPyramid& hd) {
     return hd.ptr && hd.width > 0 && hd.height > 0 && hd.levels >= 1 && hd.levels <= 16 &&
            hd.levels <= vq_mip_level_count((uint64_t)hd.width, (uint64_t)hd.height) &&
            vq_pyramid_texel_count(hd.width, hd.height, hd.levels) < (1ull << 32);
@@ -92,6 +92,25 @@ __device__ __forceinline__ void dir_to_equirect(float3 d, float& u, float& v) {
     r = a > b ? 1.57079632679f - r : r;
     // asin(t) = pi/2 - 2*atan2(a,b)  ->  v = asin(t)/pi + 0.5 = 1 - 2*r/pi
     v = fmaf(r, -2.0f / PI, 1.0f);
+}
+
+// A35: look direction of a cube texel (CubemapUtility.cpp:40-48 + 90-degree projection)
+__device__ __forceinline__ float3 cube_texel_dir(int face, int px, int py, int res) {
+    const float sx = 2.0f * ((float)px + 0.5f) / (float)res - 1.0f;
+    const float sy = 1.0f - 2.0f * ((float)py + 0.5f) / (float)res;
+    switch (face) {
+        case 0: return f3(1.0f, sy, -sx);
+        case 1: return f3(-1.0f, sy, sx);
+        case 2: return f3(sx, 1.0f, -sy);
+        case 3: return f3(sx, -1.0f, sy);
+        case 4: return f3(sx, sy, 1.0f);
+        default: return f3(-sx, sy, -1.0f);
+    }
+}
+// exact normalize (v / sqrt(dot)) for the texel basis: it feeds every sample of the texel
+__device__ __forceinline__ float3 normalize_exact(float3 v) {
+    const float l = sqrtf(dot(v, v));
+    return f3(v.x / l, v.y / l, v.z / l);
 }
 
 #endif  // __CUDACC__

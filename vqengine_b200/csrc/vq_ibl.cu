@@ -32,30 +32,11 @@ __global__ void __launch_bounds__(256) hdri_min_mip_kernel(const float4* __restr
     const float4 a = ld_stream(r0), b = ld_stream(r0 + 1), c = ld_stream(r1), d = ld_stream(r1 + 1);
     // min(rgb[0], min(rgb[1], min(rgb[2], rgb[3]))), samples ordered (0,0),(1,0),(0,1),(1,1)
     float4 o;
-    o.x = fminf(a.x, fminf(b.x, fminf(c.x, d.x)));
-    o.y = fminf(a.y, fminf(b.y, fminf(c.y, d.y)));
-    o.z = fminf(a.z, fminf(b.z, fminf(c.z, d.z)));
+    o.x = min4_ref(a.x, b.x, c.x, d.x);
+    o.y = min4_ref(a.y, b.y, c.y, d.y);
+    o.z = min4_ref(a.z, b.z, c.z, d.z);
     o.w = 1.0f;
     dst[(size_t)y * dstW + x] = o;
-}
-
-// A35: look direction of a cube texel (CubemapUtility.cpp:40-48 + 90-degree projection)
-__device__ __forceinline__ float3 cube_texel_dir(int face, int px, int py, int res) {
-    const float sx = 2.0f * ((float)px + 0.5f) / (float)res - 1.0f;
-    const float sy = 1.0f - 2.0f * ((float)py + 0.5f) / (float)res;
-    switch (face) {
-        case 0: return f3(1.0f, sy, -sx);
-        case 1: return f3(-1.0f, sy, sx);
-        case 2: return f3(sx, 1.0f, -sy);
-        case 3: return f3(sx, -1.0f, sy);
-        case 4: return f3(sx, sy, 1.0f);
-        default: return f3(-sx, sy, -1.0f);
-    }
-}
-// exact normalize (v / sqrt(dot)) for the texel basis: it feeds every sample of the texel
-__device__ __forceinline__ float3 normalize_exact(float3 v) {
-    const float l = sqrtf(dot(v, v));
-    return f3(v.x / l, v.y / l, v.z / l);
 }
 
 // =============================================================================================

@@ -772,7 +772,8 @@ extern "C" int vq_fsr_easu(VqContext* ctx, const uint32_t con[16], int address_m
 // shuffles; levels 5-6 go through 1 KB of shared memory. A global ticket (atomicAdd + __threadfence)
 // elects the last block, which reduces level 6 -> 7..12 out of shared memory.
 // Operand order per level (SURVEY.md §9): levels 1 and 7 sum (x,y),(x,y+1),(x+1,y),(x+1,y+1);
-// every other level sums (x,y),(x+1,y),(x,y+1),(x+1,y+1).
+// every other level sums (x,y),(x+1,y),(x,y+1),(x+1,y+1). The MIN instantiation (K11) takes every level row-major, the
+// order of the CPU filter it restates.
 // =============================================================================================
 struct SpdLevels { float4* p[12]; int w[12], h[12], pitch4[12]; };
 
@@ -785,8 +786,8 @@ __device__ __forceinline__ float4 spd_reduce4(float4 v0, float4 v1, float4 v2, f
     if (OP == SPD_AVG)
         return make_float4(((v0.x + v1.x) + v2.x + v3.x) * 0.25f, ((v0.y + v1.y) + v2.y + v3.y) * 0.25f,
                            ((v0.z + v1.z) + v2.z + v3.z) * 0.25f, ((v0.w + v1.w) + v2.w + v3.w) * 0.25f);
-    return make_float4(fminf(v0.x, fminf(v1.x, fminf(v2.x, v3.x))), fminf(v0.y, fminf(v1.y, fminf(v2.y, v3.y))),
-                       fminf(v0.z, fminf(v1.z, fminf(v2.z, v3.z))), 1.0f);
+    // MIN: v0..v3 in row-major order (x,y),(x+1,y),(x,y+1),(x+1,y+1) on every level (min4_ref depends on the order)
+    return make_float4(min4_ref(v0.x, v1.x, v2.x, v3.x), min4_ref(v0.y, v1.y, v2.y, v3.y), min4_ref(v0.z, v1.z, v2.z, v3.z), 1.0f);
 }
 __device__ __forceinline__ float4 shfl4(float4 v, int lane) {
     return make_float4(__shfl_sync(0xffffffffu, v.x, lane), __shfl_sync(0xffffffffu, v.y, lane),
@@ -827,7 +828,8 @@ __global__ void __launch_bounds__(256) spd_kernel(ImgV src, SpdLevels L, int mip
     for (int j = 0; j < 2; ++j)
 #pragma unroll
         for (int i = 0; i < 2; ++i) {
-            l1[j][i] = spd_reduce4<OP>(t[2 * j][2 * i], t[2 * j + 1][2 * i], t[2 * j][2 * i + 1], t[2 * j + 1][2 * i + 1]);
+            l1[j][i] = OP == SPD_AVG ? spd_reduce4<OP>(t[2 * j][2 * i], t[2 * j + 1][2 * i], t[2 * j][2 * i + 1], t[2 * j + 1][2 * i + 1])
+                                     : spd_reduce4<OP>(t[2 * j][2 * i], t[2 * j][2 * i + 1], t[2 * j + 1][2 * i], t[2 * j + 1][2 * i + 1]);
             spd_store(L, 1, mips, tileX * 32 + px * 2 + i, tileY * 32 + py * 2 + j, l1[j][i]);
         }
     if (mips <= 1) return;
@@ -880,7 +882,7 @@ __global__ void __launch_bounds__(256) spd_kernel(ImgV src, SpdLevels L, int mip
         const float4 v1 = __ldcg(p6 + (size_t)(2 * y + 1) * pitch6 + 2 * x);
         const float4 v2 = __ldcg(p6 + (size_t)(2 * y) * pitch6 + 2 * x + 1);
         const float4 v3 = __ldcg(p6 + (size_t)(2 * y + 1) * pitch6 + 2 * x + 1);
-        const float4 v = spd_reduce4<OP>(v0, v1, v2, v3);
+        const float4 v = OP == SPD_AVG ? spd_reduce4<OP>(v0, v1, v2, v3) : spd_reduce4<OP>(v0, v2, v1, v3);
         spd_store(L, 7, mips, x, y, v);
         sTail[y * 32 + x] = v;
     }
