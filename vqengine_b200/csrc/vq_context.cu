@@ -28,6 +28,25 @@ int vq_check_launch(const char* what) {
     return VQ_OK;
 }
 
+// The one place context scratch grows. A launch enqueued by an earlier call, on any stream, may still be reading the old
+// buffer (e.g. K1 on another stream reading the sampling copies), so the whole device is drained before it is released.
+// The contents do not survive a regrow. Once a renderer's sizes are fixed no call regrows, so steady frames never wait here.
+int vq_scratch_reserve(VqScratch& s, size_t need, const char* what) {
+    if (s.bytes >= need) return VQ_OK;
+    if (s.p) {
+        VQ_CUDA_OK(cudaDeviceSynchronize());
+        cudaFree(s.p);
+        s.p = nullptr; s.bytes = 0;
+    }
+    if (cudaMalloc(&s.p, need) != cudaSuccess) {
+        cudaGetLastError(); s.p = nullptr;
+        vq_set_error("cudaMalloc(%zu) failed (%s)", need, what);
+        return VQ_ERR_OUT_OF_MEMORY;
+    }
+    s.bytes = need;
+    return VQ_OK;
+}
+
 int vq_fill_peer_sync(const VqPeerSignal* sig, PeerSync* out) {
     memset(out, 0, sizeof(*out));
     if (!sig || sig->n_ranks <= 1) return VQ_OK;
@@ -63,7 +82,6 @@ int vq_ctx_create(int device, VqContext** out_ctx) {
     }
     VqContext* c = new (std::nothrow) VqContext();
     if (!c) return VQ_ERR_OUT_OF_MEMORY;
-    memset(c, 0, sizeof(*c));
     c->device = device;
     c->sm_count = prop.multiProcessorCount;
     c->l2_bytes = prop.l2CacheSize;
@@ -82,35 +100,9 @@ int vq_ctx_destroy(VqContext* ctx) {
         for (auto& s : ctx->streams) cudaStreamDestroy(s);
         for (auto& e : ctx->events) cudaEventDestroy(e);
     }
-    if (ctx->stage_dev) cudaFree(ctx->stage_dev);
-    for (void* p : {ctx->env_all, ctx->tmp_diff, ctx->tmp_spec, ctx->tmp_lut, ctx->resize_mid, ctx->resize_tab, ctx->depth_pad, ctx->shadow_rec}) if (p) cudaFree(p);
     if (ctx->spd_counter) cudaFree(ctx->spd_counter);
     delete ctx->spd_next; delete ctx->mu;
-    delete ctx;
-    return VQ_OK;
-}
-
-static int ctx_resize_locked(VqContext* ctx, int width, int height);
-int vq_ctx_resize(VqContext* ctx, int width, int height) {
-    int rc = vq_enter(ctx); if (rc) return rc;
-    VqScratchLock lock(ctx);
-    return ctx_resize_locked(ctx, width, height);
-}
-int vq_ctx_resize_locked(VqContext* ctx, int width, int height) { return ctx_resize_locked(ctx, width, height); }
-static int ctx_resize_locked(VqContext* ctx, int width, int height) {
-    VQ_REQUIRE(width > 0 && height > 0, "resolution must be positive");
-    const size_t need = (size_t)width * height * 16 * 4;   // 3 G-buffer planes + output
-    if (ctx->stage_dev_bytes < need) {
-        if (ctx->stage_dev) cudaFree(ctx->stage_dev);
-        ctx->stage_dev = nullptr; ctx->stage_dev_bytes = 0;
-        if (cudaMalloc(&ctx->stage_dev, need) != cudaSuccess) { cudaGetLastError(); vq_set_error("staging cudaMalloc(%zu) failed", need); return VQ_ERR_OUT_OF_MEMORY; }
-        ctx->stage_dev_bytes = need;
-    }
-    if (!ctx->streams_ready) {
-        for (auto& s : ctx->streams) VQ_CUDA_OK(cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking));
-        for (auto& e : ctx->events) VQ_CUDA_OK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-        ctx->streams_ready = 1;
-    }
+    delete ctx;                 // frees the scratch (~VqScratch)
     return VQ_OK;
 }
 

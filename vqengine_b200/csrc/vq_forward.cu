@@ -803,13 +803,26 @@ int footprint_lut(const VqImage& lut, float4* dst, cudaStream_t stream) {
     return vq_check_launch("lut_footprint");
 }
 
-int ensure_bytes(void** ptr, size_t* have, size_t need) {
-    if (*have >= need && *ptr) return VQ_OK;
-    if (*ptr) cudaFree(*ptr);
-    *ptr = nullptr; *have = 0;
-    if (cudaMalloc(ptr, need) != cudaSuccess) { cudaGetLastError(); vq_set_error("cudaMalloc(%zu) failed", need); return VQ_ERR_OUT_OF_MEMORY; }
-    *have = need;
-    return VQ_OK;
+// K1's sampling copies of one environment share ONE buffer: diffuse | specular | LUT footprints, each part 256-byte aligned
+// (the specular cube and the LUT only when asked). Points the views into the buffer at `base` and returns its size.
+size_t sampling_views(const VqEnvironmentMaps& env, bool withSpec, bool withLut, uintptr_t base, CubeV& diff, CubeV& spec, LutV& lut) {
+    auto up = [](size_t b) { return (b + 255) & ~(size_t)255; };
+    const size_t bD = up(padded_bytes(env.irradiance_diffuse.res, env.irradiance_diffuse.mips));
+    const size_t bS = withSpec ? up(padded_bytes(env.irradiance_specular.res, env.irradiance_specular.mips)) : 0;
+    fill_cube_view(env.irradiance_diffuse, (const float4*)base, diff);
+    if (withSpec) fill_cube_view(env.irradiance_specular, (const float4*)(base + bD), spec);
+    if (withLut) lut.q = (const float4*)(base + bD + bS);
+    return bD + bS + (withLut ? up(lut_footprint_bytes(env.brdf_lut)) : 0);
+}
+// grows `s` to that layout, builds the copies of `env` into it on `stream` and points the views at them
+int build_sampling_copies(VqScratch& s, const VqEnvironmentMaps& env, bool withSpec, bool withLut, cudaStream_t stream,
+                          CubeV& diff, CubeV& spec, LutV& lut) {
+    int rc = vq_scratch_reserve(s, sampling_views(env, withSpec, withLut, 0, diff, spec, lut), "sampling copies"); if (rc) return rc;
+    sampling_views(env, withSpec, withLut, (uintptr_t)s.p, diff, spec, lut);
+    rc = pad_cube(env.irradiance_diffuse, (float4*)diff.p, stream);
+    if (!rc && withSpec) rc = pad_cube(env.irradiance_specular, (float4*)spec.p, stream);
+    if (!rc && withLut) rc = footprint_lut(env.brdf_lut, (float4*)lut.q, stream);
+    return rc;
 }
 
 }  // namespace
@@ -887,7 +900,7 @@ int vq_forward_launch_multi(VqContext* ctx, const VqPerFrameData* pf, const VqPe
                L.numSpotCasters >= 0 && L.numSpotCasters <= VQ_NUM_SHADOWING_LIGHTS_SPOT, "light counts exceed the cbuffer arrays");
     VQ_REQUIRE(row_begin < row_end || !(sig && sig->n_ranks > 1), "a rendezvous needs a non-empty row range (the kernel runs it)");
     if (row_begin == row_end) return VQ_OK;
-    VqScratchLock lock(ctx);           // env_* registration and the per-call tmp_* sampling copies are the context's
+    VqScratchLock lock(ctx);           // the registered environment and the per-call sampling copies are the context's
 
     FwdParams P;
     memset(&P, 0, sizeof(P));
@@ -912,29 +925,16 @@ int vq_forward_launch_multi(VqContext* ctx, const VqPerFrameData* pf, const VqPe
         VQ_REQUIRE(env->brdf_lut.width <= 8192 && env->brdf_lut.height <= 8192, "BRDF LUT larger than 8192^2");
         P.lut.w = env->brdf_lut.width; P.lut.h = env->brdf_lut.height;
     }
-    // bordered sampling copies: from the prepared environment when it matches, else padded now on this stream
+    // bordered sampling copies: from the prepared environment when it matches (the descriptors checked above are non-null, so
+    // a match also means the registration holds every part this call reads), else built now on this stream
     int rc;
+    const bool full = !P.diffuseOnly;
     const bool prepared = ctx->env_valid && same_cube(ctx->env_key.irradiance_diffuse, env->irradiance_diffuse) &&
                           (P.diffuseOnly || (same_cube(ctx->env_key.irradiance_specular, env->irradiance_specular) &&
-                                             same_image(ctx->env_key.brdf_lut, env->brdf_lut) && ctx->env_lut));
-    if (prepared) {
-        fill_cube_view(env->irradiance_diffuse, (const float4*)ctx->env_diff, P.diff);
-        if (!P.diffuseOnly) {
-            fill_cube_view(env->irradiance_specular, (const float4*)ctx->env_spec, P.spec);
-            P.lut.q = (const float4*)ctx->env_lut;
-        }
-    } else {
-        rc = ensure_bytes(&ctx->tmp_diff, &ctx->tmp_diff_bytes, padded_bytes(env->irradiance_diffuse.res, env->irradiance_diffuse.mips)); if (rc) return rc;
-        rc = pad_cube(env->irradiance_diffuse, (float4*)ctx->tmp_diff, stream); if (rc) return rc;
-        fill_cube_view(env->irradiance_diffuse, (const float4*)ctx->tmp_diff, P.diff);
-        if (!P.diffuseOnly) {
-            rc = ensure_bytes(&ctx->tmp_spec, &ctx->tmp_spec_bytes, padded_bytes(env->irradiance_specular.res, env->irradiance_specular.mips)); if (rc) return rc;
-            rc = pad_cube(env->irradiance_specular, (float4*)ctx->tmp_spec, stream); if (rc) return rc;
-            fill_cube_view(env->irradiance_specular, (const float4*)ctx->tmp_spec, P.spec);
-            rc = ensure_bytes(&ctx->tmp_lut, &ctx->tmp_lut_bytes, lut_footprint_bytes(env->brdf_lut)); if (rc) return rc;
-            rc = footprint_lut(env->brdf_lut, (float4*)ctx->tmp_lut, stream); if (rc) return rc;
-            P.lut.q = (const float4*)ctx->tmp_lut;
-        }
+                                             same_image(ctx->env_key.brdf_lut, env->brdf_lut)));
+    if (prepared) sampling_views(*env, full, full, (uintptr_t)ctx->env_prepared.p, P.diff, P.spec, P.lut);
+    else {
+        rc = build_sampling_copies(ctx->env_per_call, *env, full, full, stream, P.diff, P.spec, P.lut); if (rc) return rc;
     }
     P.rowBegin = row_begin; P.rows = row_end - row_begin; P.width = W;
     const bool shadowed = shadow && shadow->p;
@@ -1032,20 +1032,9 @@ extern "C" int vq_environment_prepare(VqContext* ctx, const VqEnvironmentMaps* e
     const bool hasSpec = env->irradiance_specular.ptr != nullptr, hasLut = env->brdf_lut.ptr != nullptr;
     if (hasSpec) VQ_REQUIRE(cube_desc_ok(env->irradiance_specular), "bad cubemap descriptor (irradiance_specular)");
     if (hasLut) VQ_REQUIRE(vq_image_ok(env->brdf_lut, 8) && env->brdf_lut.width <= 8192 && env->brdf_lut.height <= 8192, "bad BRDF LUT descriptor");
-    // ONE allocation for the three sampling copies (diffuse | specular | LUT footprints, 256-byte aligned parts): one buffer
-    // to grow and free instead of three
-    auto up = [](size_t b) { return (b + 255) & ~(size_t)255; };
-    const size_t bD = up(padded_bytes(env->irradiance_diffuse.res, env->irradiance_diffuse.mips));
-    const size_t bS = hasSpec ? up(padded_bytes(env->irradiance_specular.res, env->irradiance_specular.mips)) : 0;
-    const size_t bL = hasLut ? up(lut_footprint_bytes(env->brdf_lut)) : 0;
-    rc = ensure_bytes(&ctx->env_all, &ctx->env_all_bytes, bD + bS + bL); if (rc) return rc;
-    ctx->env_diff = ctx->env_all;
-    ctx->env_spec = hasSpec ? (char*)ctx->env_all + bD : nullptr;
-    ctx->env_lut = hasLut ? (char*)ctx->env_all + bD + bS : nullptr;
-    rc = pad_cube(env->irradiance_diffuse, (float4*)ctx->env_diff, (cudaStream_t)stream); if (rc) return rc;
+    CubeV diff, spec; LutV lut;        // not kept: a call that matches the registration points its own views (sampling_views)
+    rc = build_sampling_copies(ctx->env_prepared, *env, hasSpec, hasLut, (cudaStream_t)stream, diff, spec, lut); if (rc) return rc;
     ctx->env_key = *env;
-    if (hasSpec) { rc = pad_cube(env->irradiance_specular, (float4*)ctx->env_spec, (cudaStream_t)stream); if (rc) return rc; }
-    if (hasLut) { rc = footprint_lut(env->brdf_lut, (float4*)ctx->env_lut, (cudaStream_t)stream); if (rc) return rc; }
     ctx->env_valid = 1;
     return VQ_OK;
 }

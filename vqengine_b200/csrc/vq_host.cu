@@ -1,8 +1,26 @@
 // vq_host.cu — blocking host-buffer entry point for K1: the call an engine integration makes when its
 // frame data lives in system memory. Rows are cut into chunks and pipelined over three streams
 // (upload | shade | download) so that PCIe traffic in both directions overlaps the kernel; with pinned
-// host memory (cudaHostRegister / cudaMallocHost) the copies are truly asynchronous.
+// host memory (cudaHostRegister / cudaMallocHost) the copies are truly asynchronous. vq_ctx_resize pre-sizes its staging.
 #include "vq_common.cuh"
+
+// the pipeline's three streams and event ring, created on first use (caller holds the scratch lock)
+static int host_streams(VqContext* ctx) {
+    if (!ctx->streams_ready) {
+        for (auto& s : ctx->streams) VQ_CUDA_OK(cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking));
+        for (auto& e : ctx->events) VQ_CUDA_OK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+        ctx->streams_ready = 1;
+    }
+    return VQ_OK;
+}
+
+extern "C" int vq_ctx_resize(VqContext* ctx, int width, int height) {
+    int rc = vq_enter(ctx); if (rc) return rc;
+    VQ_REQUIRE(width > 0 && height > 0, "resolution must be positive");
+    VqScratchLock lock(ctx);
+    rc = host_streams(ctx); if (rc) return rc;
+    return vq_scratch_reserve(ctx->stage, (size_t)width * height * 16 * 4, "host-call staging");   // 3 G-buffer planes + output
+}
 
 extern "C" int vq_forward_lighting_host(VqContext* ctx, const VqPerFrameData* pf, const VqPerViewLightingData* pv,
                                         const VqGBuffer* hgb, const VqEnvironmentMaps* denv, VqImage hout) {
@@ -23,16 +41,9 @@ extern "C" int vq_forward_lighting_host(VqContext* ctx, const VqPerFrameData* pf
     const int planes = hasEm ? 5 : 4;
     const size_t rowBytes = (size_t)W * 16, planeBytes = rowBytes * H;
     VqScratchLock lock(ctx);           // the staging buffer, the three streams and the event ring are the context's
-    if (ctx->stage_dev_bytes < planeBytes * planes || !ctx->streams_ready) {
-        // (re)size staging: vq_ctx_resize sizes for 4 planes; grow here if an emissive plane is present
-        rc = vq_ctx_resize_locked(ctx, W, H); if (rc) return rc;
-        if (ctx->stage_dev_bytes < planeBytes * planes) {
-            cudaFree(ctx->stage_dev); ctx->stage_dev = nullptr; ctx->stage_dev_bytes = 0;
-            if (cudaMalloc(&ctx->stage_dev, planeBytes * planes) != cudaSuccess) { cudaGetLastError(); vq_set_error("staging cudaMalloc failed"); return VQ_ERR_OUT_OF_MEMORY; }
-            ctx->stage_dev_bytes = planeBytes * planes;
-        }
-    }
-    char* base = (char*)ctx->stage_dev;
+    rc = host_streams(ctx); if (rc) return rc;
+    rc = vq_scratch_reserve(ctx->stage, planeBytes * planes, "host-call staging"); if (rc) return rc;
+    char* base = (char*)ctx->stage.p;
     VqGBuffer dgb;
     dgb.position_ao      = VqImage{base + 0 * planeBytes, W, H, rowBytes};
     dgb.normal_roughness = VqImage{base + 1 * planeBytes, W, H, rowBytes};

@@ -129,15 +129,6 @@ __global__ void __launch_bounds__(256) depth_min6_kernel(const __grid_constant__
     }
 }
 
-int ensure_scratch(void** ptr, size_t* have, size_t need) {
-    if (*have >= need && *ptr) return VQ_OK;
-    if (*ptr) cudaFree(*ptr);
-    *ptr = nullptr; *have = 0;
-    if (cudaMalloc(ptr, need) != cudaSuccess) { cudaGetLastError(); vq_set_error("cudaMalloc(%zu) failed", need); return VQ_ERR_OUT_OF_MEMORY; }
-    *have = need;
-    return VQ_OK;
-}
-
 }  // namespace
 
 extern "C" int vq_forward_lighting_shadowed(VqContext* ctx, const VqPerFrameData* pf, const VqPerViewLightingData* pv,
@@ -168,8 +159,8 @@ extern "C" int vq_forward_lighting_shadowed(VqContext* ctx, const VqPerFrameData
     P.rowBegin = row_begin; P.rows = row_end - row_begin; P.width = gb->position_ao.width;
     vqshadow::fill_shadow_lights(P.L, *pf, *pv, *sm);
     VqScratchLock lock(ctx);                       // the records are context scratch (vqcuda.h lists the call as not re-entrant per context)
-    rc = ensure_scratch(&ctx->shadow_rec, &ctx->shadow_rec_bytes, (size_t)P.width * P.rows * sizeof(uint2)); if (rc) return rc;
-    P.rec = (uint2*)ctx->shadow_rec; P.recPitch = P.width;
+    rc = vq_scratch_reserve(ctx->shadow_rec, (size_t)P.width * P.rows * sizeof(uint2), "PCF records"); if (rc) return rc;
+    P.rec = (uint2*)ctx->shadow_rec.p; P.recPitch = P.width;
 
     const unsigned gx = (unsigned)((P.width + 127) / 128);
     unsigned gy = (unsigned)(ctx->sm_count * PCF_MIN_BLOCKS) / gx;
@@ -206,8 +197,8 @@ extern "C" int vq_depth_min_pyramid(VqContext* ctx, VqImage depth, void* levels,
     // padded-domain copies of levels 6 and 12 (what a following launch reads): level 6 is at most ceil(W/64) x ceil(H/64)
     const size_t padTexels = (size_t)((W + 63) / 64) * ((H + 63) / 64);
     VqScratchLock lock(ctx);
-    rc = ensure_scratch(&ctx->depth_pad, &ctx->depth_pad_bytes, padTexels * 2 * 4 > 16 ? padTexels * 2 * 4 : 16); if (rc) return rc;
-    float* pads[2] = {(float*)ctx->depth_pad, (float*)ctx->depth_pad + padTexels};
+    rc = vq_scratch_reserve(ctx->depth_pad, padTexels * 2 * 4 > 16 ? padTexels * 2 * 4 : 16, "depth pyramid pads"); if (rc) return rc;
+    float* pads[2] = {(float*)ctx->depth_pad.p, (float*)ctx->depth_pad.p + padTexels};
     float* out = (float*)levels;
     DepthArgs A;
     A.src = (const float*)depth.ptr; A.srcPitch = (int)(depth.pitch_bytes / 4); A.sw = W; A.sh = H;
