@@ -6,7 +6,7 @@
 //   mbarrier ring in shared memory, the result leaves as one STG.128 per pixel; one thread shades TWO pixels (two
 //   independent dependency chains through the light loop); the light array is staged once per
 //   CTA into shared memory; the IBL cubemaps and the BRDF LUT are gathered from L2-resident sampling copies
-//   (bordered texels / footprint records, 68 MB at the reference sizes) with five 32-byte gathers per pixel, each read by
+//   (bordered texels / LUT column pairs, 51 MB at the reference sizes) with five 32-byte gathers per pixel, each read by
 //   two neighbouring lanes together (see "lane-pair record gathers"), because the L1 data pipe — one wavefront per distinct
 //   line of a divergent gather — is what bounds this kernel (DESIGN.md §4).
 // The math is PSMain's with per-pixel invariants hoisted out of the light loops (N, V, N.V, the
@@ -32,10 +32,11 @@ namespace {
 // together (cube_issue / ldg_pair), the even lane t(i) and the odd lane t(i+1), so one instruction touches at most 16 places
 // (a row crosses a line boundary once in 8 positions). mipOffset[] are position offsets of face 0 per mip.
 struct CubeV { const float4* p; int res, mips; uint32_t mipOffset[16]; };
-// Footprint copy of the BRDF LUT: record (cx,cy), cx = clamp(x0+1, 0, W), holds the CLAMP-addressed 2x2 footprint
-// {p(x0,y0), p(x0+1,y0), p(x0,y0+1), p(x0+1,y0+1)} as 4 x float2 = 32 bytes: one record (one sector) per pixel, half .a the
-// row y0 and half .b the row y0+1, read by a lane pair like a row of a cube footprint.
-struct LutV { const float4* q; int w, h; };
+// Column-pair copy of the BRDF LUT: a (W+2) x (H+1) grid of 16-byte texels, texel (c,cy) = {p(xc,y0), p(xc,y1)} with
+// xc = clamp(c-1, 0, W-1), y0 = clamp(cy-1, 0, H-1), y1 = clamp(cy, 0, H-1). The CLAMP-addressed bilinear footprint of (x0,y0) is
+// then texels c = x0+1 and x0+2 of row cy = y0+1: 32 contiguous bytes, read by a lane pair exactly like a row of a cube footprint.
+// 16 bytes per footprint position keep the copies small enough for L2 to hold most of them (DESIGN.md §9).
+struct LutV { const float4* p; int w, h; };
 struct F8 { float4 a, b; };
 
 struct SPoint { float3 pos; float d2Limit; float3 color; float brightness; };
@@ -148,16 +149,14 @@ __global__ void __launch_bounds__(256) cube_pad_kernel(const float4* __restrict_
         dst[idx] = bordered_texel(src, res, mips, idx);
 }
 
-// BRDF LUT (float2, pitched) -> footprint records (see LutV): (W+1) x (H+1) records of 32 bytes
-__global__ void __launch_bounds__(256) lut_footprint_kernel(const float2* __restrict__ src, int pitch2, int W, int H, float4* __restrict__ dst) {
-    const uint32_t total = (uint32_t)(W + 1) * (uint32_t)(H + 1);
+// BRDF LUT (float2, pitched) -> column pairs (see LutV): (W+2) x (H+1) texels of 16 bytes
+__global__ void __launch_bounds__(256) lut_pair_kernel(const float2* __restrict__ src, int pitch2, int W, int H, float4* __restrict__ dst) {
+    const uint32_t total = (uint32_t)(W + 2) * (uint32_t)(H + 1);
     for (uint32_t idx = blockIdx.x * 256u + threadIdx.x; idx < total; idx += gridDim.x * 256u) {
-        const int cx = (int)(idx % (uint32_t)(W + 1)), cy = (int)(idx / (uint32_t)(W + 1));
-        const int x0 = max(cx - 1, 0), x1 = min(cx, W - 1), y0 = max(cy - 1, 0), y1 = min(cy, H - 1);
-        const float2 p00 = __ldg(src + (size_t)y0 * pitch2 + x0), p10 = __ldg(src + (size_t)y0 * pitch2 + x1);
-        const float2 p01 = __ldg(src + (size_t)y1 * pitch2 + x0), p11 = __ldg(src + (size_t)y1 * pitch2 + x1);
-        dst[2 * (size_t)idx] = make_float4(p00.x, p00.y, p10.x, p10.y);
-        dst[2 * (size_t)idx + 1] = make_float4(p01.x, p01.y, p11.x, p11.y);
+        const int c = (int)(idx % (uint32_t)(W + 2)), cy = (int)(idx / (uint32_t)(W + 2));
+        const int xc = min(max(c - 1, 0), W - 1), y0 = max(cy - 1, 0), y1 = min(cy, H - 1);
+        const float2 p0 = __ldg(src + (size_t)y0 * pitch2 + xc), p1 = __ldg(src + (size_t)y1 * pitch2 + xc);
+        dst[idx] = make_float4(p0.x, p0.y, p1.x, p1.y);
     }
 }
 
@@ -443,7 +442,7 @@ __device__ __forceinline__ float4 ldg128(const float4* p) {
     return r;
 }
 // ---- lane-pair record gathers ----
-// A record here is the 32 bytes one bilinear row needs: two adjacent cube texels, or a LUT footprint (one sector). sm_90 has no
+// A record here is the 32 bytes one bilinear row needs: two adjacent texels of a cube or of the LUT's column pairs. sm_90 has no
 // 256-bit load, so a record takes two LDG.128. If every lane read its own record with both, each instruction would touch up to 32
 // unrelated lines and every line would be paid for twice. So lanes 2q and 2q+1 read their two records TOGETHER: in one
 // instruction both read the even lane's record (the even lane its half .a, the odd lane its half .b), in the other both read the
@@ -452,12 +451,10 @@ __device__ __forceinline__ float4 ldg128(const float4* p) {
 // per component swaps the .b halves. Every lane of the warp takes part (pixels off a ragged row are aliased, never masked off),
 // so the shuffles use the full mask.
 __device__ __forceinline__ bool odd_lane() { return (threadIdx.x & 1u) != 0u; }
-// record k starts at float4 index STRIDE*k: STRIDE 1 for a cube (record = texel k and its right neighbour), 2 for the LUT.
+// record k = texel k and its right neighbour.
 // iE, iO: float4 indices of what this lane reads of the even lane's record (.a on an even lane, .b on an odd one) and of the odd
-// lane's record (.b on an even lane, .a on an odd one), given this lane's record `rec`
-template <uint32_t STRIDE>
-__device__ __forceinline__ void pair_halves(uint32_t rec, uint32_t& iE, uint32_t& iO) {
-    const uint32_t mine = STRIDE * rec;
+// lane's record (.b on an even lane, .a on an odd one), given this lane's record `mine`
+__device__ __forceinline__ void pair_halves(uint32_t mine, uint32_t& iE, uint32_t& iO) {
     const uint32_t other = __shfl_xor_sync(0xffffffffu, mine, 1) + 1u;          // the partner's record, second half
     const bool odd = odd_lane();
     iE = odd ? other : mine; iO = odd ? mine : other;
@@ -495,9 +492,9 @@ __device__ __forceinline__ CubeLoad cube_issue(const float4* __restrict__ texels
     L.fx = x - xf; L.fy = y - yf;
     const uint32_t off = min(f.base + (uint32_t)((int)yf + 1) * f.P + (uint32_t)((int)xf + 1), maxRec);
     uint32_t e0, o0, e1, o1;
-    pair_halves<1u>(off, e0, o0);
+    pair_halves(off, e0, o0);
     if (UNIFORM_P) { e1 = e0 + f.P; o1 = o0 + f.P; }
-    else pair_halves<1u>(off + f.P, e1, o1);
+    else pair_halves(off + f.P, e1, o1);
     L.r0 = ldg_pair(texels, e0, o0); L.r1 = ldg_pair(texels, e1, o1);
     return L;
 }
@@ -518,16 +515,17 @@ __device__ __forceinline__ LutLoad lut_issue(const LutV& l, float u, float v) { 
     const float x0 = floorf(x), y0 = floorf(y);
     LutLoad L;
     L.fx = x - x0; L.fy = y - y0;
+    // clamped per axis: the footprint's two texels lie inside the copy for every input, NaN and inf included
     const int cx = min(max((int)x0 + 1, 0), l.w), cy = min(max((int)y0 + 1, 0), l.h);
     uint32_t e, o;
-    pair_halves<2u>((uint32_t)(cy * (l.w + 1) + cx), e, o);
-    L.q = ldg_pair(l.q, e, o);
+    pair_halves((uint32_t)(cy * (l.w + 2) + cx), e, o);
+    L.q = ldg_pair(l.p, e, o);
     return L;
 }
-__device__ __forceinline__ float2 lut_finish(const LutLoad& L) {    // record = {p00, p10 | p01, p11} as float2 each
+__device__ __forceinline__ float2 lut_finish(const LutLoad& L) {    // record = {p00, p01 | p10, p11} as float2 each
     const F8 q = own_record<4>(L.q);
     const f2 fx = bc(L.fx), fy = bc(L.fy);
-    const f2 p00 = mk(q.a.x, q.a.y), p10 = mk(q.a.z, q.a.w), p01 = mk(q.b.x, q.b.y), p11 = mk(q.b.z, q.b.w);
+    const f2 p00 = mk(q.a.x, q.a.y), p01 = mk(q.a.z, q.a.w), p10 = mk(q.b.x, q.b.y), p11 = mk(q.b.z, q.b.w);
     const f2 t = fma2(fx, p10 - p00, p00), u = fma2(fx, p11 - p01, p01);
     return fma2(fy, u - t, t).v;
 }
@@ -793,17 +791,18 @@ void fill_cube_view(const VqCubemap& c, const float4* padded, CubeV& v) {
 }
 bool same_cube(const VqCubemap& a, const VqCubemap& b) { return a.ptr == b.ptr && a.res == b.res && a.mips == b.mips; }
 bool same_image(const VqImage& a, const VqImage& b) { return a.ptr == b.ptr && a.width == b.width && a.height == b.height && a.pitch_bytes == b.pitch_bytes; }
-size_t lut_footprint_bytes(const VqImage& lut) { return (size_t)(lut.width + 1) * (size_t)(lut.height + 1) * 32; }
-// builds the footprint copy of the BRDF LUT into `dst` on `stream`
-int footprint_lut(const VqImage& lut, float4* dst, cudaStream_t stream) {
-    const uint32_t total = (uint32_t)(lut.width + 1) * (uint32_t)(lut.height + 1);
+// no slack needed: lut_issue clamps both coordinates, so no footprint can start past texel (W, H) of the copy
+size_t lut_pair_bytes(const VqImage& lut) { return (size_t)(lut.width + 2) * (size_t)(lut.height + 1) * 16; }
+// builds the column-pair copy of the BRDF LUT into `dst` on `stream`
+int pair_lut(const VqImage& lut, float4* dst, cudaStream_t stream) {
+    const uint32_t total = (uint32_t)(lut.width + 2) * (uint32_t)(lut.height + 1);
     unsigned blocks = (total + 255u) / 256u;
     if (blocks > 148u * 16u) blocks = 148u * 16u;
-    lut_footprint_kernel<<<blocks, 256, 0, stream>>>((const float2*)lut.ptr, (int)(lut.pitch_bytes / 8), lut.width, lut.height, dst);
-    return vq_check_launch("lut_footprint");
+    lut_pair_kernel<<<blocks, 256, 0, stream>>>((const float2*)lut.ptr, (int)(lut.pitch_bytes / 8), lut.width, lut.height, dst);
+    return vq_check_launch("lut_pair");
 }
 
-// K1's sampling copies of one environment share ONE buffer: diffuse | specular | LUT footprints, each part 256-byte aligned
+// K1's sampling copies of one environment share ONE buffer: diffuse | specular | LUT column pairs, each part 256-byte aligned
 // (the specular cube and the LUT only when asked). Points the views into the buffer at `base` and returns its size.
 size_t sampling_views(const VqEnvironmentMaps& env, bool withSpec, bool withLut, uintptr_t base, CubeV& diff, CubeV& spec, LutV& lut) {
     auto up = [](size_t b) { return (b + 255) & ~(size_t)255; };
@@ -811,8 +810,8 @@ size_t sampling_views(const VqEnvironmentMaps& env, bool withSpec, bool withLut,
     const size_t bS = withSpec ? up(padded_bytes(env.irradiance_specular.res, env.irradiance_specular.mips)) : 0;
     fill_cube_view(env.irradiance_diffuse, (const float4*)base, diff);
     if (withSpec) fill_cube_view(env.irradiance_specular, (const float4*)(base + bD), spec);
-    if (withLut) lut.q = (const float4*)(base + bD + bS);
-    return bD + bS + (withLut ? up(lut_footprint_bytes(env.brdf_lut)) : 0);
+    if (withLut) lut.p = (const float4*)(base + bD + bS);
+    return bD + bS + (withLut ? up(lut_pair_bytes(env.brdf_lut)) : 0);
 }
 // grows `s` to that layout, builds the copies of `env` into it on `stream` and points the views at them
 int build_sampling_copies(VqScratch& s, const VqEnvironmentMaps& env, bool withSpec, bool withLut, cudaStream_t stream,
@@ -821,7 +820,7 @@ int build_sampling_copies(VqScratch& s, const VqEnvironmentMaps& env, bool withS
     sampling_views(env, withSpec, withLut, (uintptr_t)s.p, diff, spec, lut);
     rc = pad_cube(env.irradiance_diffuse, (float4*)diff.p, stream);
     if (!rc && withSpec) rc = pad_cube(env.irradiance_specular, (float4*)spec.p, stream);
-    if (!rc && withLut) rc = footprint_lut(env.brdf_lut, (float4*)lut.q, stream);
+    if (!rc && withLut) rc = pair_lut(env.brdf_lut, (float4*)lut.p, stream);
     return rc;
 }
 
