@@ -341,7 +341,10 @@ typedef struct VqMaterialTextures {
  *   position_u = { WorldSpacePosition.xyz, uv.x }
  *   normal_v   = { WorldSpaceNormal.xyz  (interpolated, not normalised), uv.y }
  *   tangent_m  = { WorldSpaceTangent.xyz (interpolated, not normalised), material index as an exact small float }
- *   ssao       = optional R32F plane, the texScreenSpaceAO the shader point-samples (NULL -> 1) */
+ *   ssao       = optional R32F plane, the texScreenSpaceAO the shader point-samples (NULL -> 1)
+ * Domain: the material index converts toward zero with NaN -> 0 and saturation, then clamps to [0, count-1]. The floored
+ * texel coordinate floor(u*W - 0.5) converts the same way and then wraps, so beyond 2^31 it reads the column of +-2^31 mod W.
+ * A texel coordinate that is not finite gives a NaN sample (also when only one level of a trilinear pair overflows). */
 typedef struct VqSurfaceInputs {
     VqImage position_u, normal_v, tangent_m;
     VqImage ssao;
@@ -360,7 +363,8 @@ VQ_API int vq_texture_build_mips(VqContext* ctx, VqTexture2D tex, void* stream);
  * all maps (like the bordered cubemap copies of vq_environment_prepare). The copy is taken HERE, synchronously (the call
  * waits for the device first, so mip chains still being built on other streams are complete): fill the textures, mips
  * included, before creating the table, and re-create the table when texels change. Costs 16 B per texel of the shared
- * size; if that allocation fails, or with VQ_SURFACE_RECORDS=0 in the environment, the maps are sampled one by one. */
+ * size; if that allocation fails, or with VQ_SURFACE_RECORDS=0 in the environment, the maps are sampled one by one.
+ * textureConfig must lie in [0, 2^31) (it is converted with (int)); anything else, NaN included, is VQ_ERR_INVALID_ARG. */
 VQ_API int vq_material_table_create(VqContext* ctx, const VqMaterialData* materials,
                                     const VqMaterialTextures* textures, int count, VqMaterialTable** out_table);
 VQ_API int vq_material_table_destroy(VqContext* ctx, VqMaterialTable* table);

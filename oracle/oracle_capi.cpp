@@ -101,7 +101,9 @@ void orc_gbuffer_from_materials(const float* position_u, const float* normal_v, 
             in.WorldSpaceNormal = make3(normal_v[o], normal_v[o + 1], normal_v[o + 2]);
             in.WorldSpaceTangent = make3(tangent_m[o], tangent_m[o + 1], tangent_m[o + 2]);
             in.uv = rawuv(x, y);
-            int mi = (int)tangent_m[o + 3];
+            // the device's conversion (cvt.rzi: NaN -> 0, saturated), then clamped; the C++ conversion is undefined there
+            const float mf = tangent_m[o + 3];
+            int mi = mf != mf ? 0 : (mf >= 2147483648.0f ? 2147483647 : (mf < -2147483648.0f ? (-2147483647 - 1) : (int)mf));
             mi = mi < 0 ? 0 : (mi >= n_materials ? n_materials - 1 : mi);
             // fine derivatives inside the aligned 2x2 quad, partner clamped to the image
             const int qx = x & ~1, qy = y & ~1;

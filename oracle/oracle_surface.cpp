@@ -44,6 +44,10 @@ void MipImage_Box8(const uint8_t* src, uint8_t* dst, int width, int height) {
 size_t Texture8::offset(int level) const { return pyramid_texel_count(width, height, level); }
 
 static inline int wrapi(int i, int n) { int r = i % n; return r < 0 ? r + n : r; }
+// the device's float -> int conversion (cvt.rzi: NaN -> 0, saturated); the C++ conversion is undefined outside the int range
+static inline int to_int_sat(float x) {
+    return x != x ? 0 : (x >= 2147483648.0f ? 2147483647 : (x < -2147483648.0f ? (-2147483647 - 1) : (int)x));
+}
 static inline float4 ld8(const uint8_t* p) {
     return {(float)p[0] / 255.0f, (float)p[1] / 255.0f, (float)p[2] / 255.0f, (float)p[3] / 255.0f};
 }
@@ -53,10 +57,11 @@ static float4 BilinearWrap8(const Texture8& tex, int level, float2 uv) {
     const uint8_t* base = tex.data + 4 * tex.offset(level);
     const float x = uv.x * (float)W - 0.5f;
     const float y = uv.y * (float)H - 0.5f;
-    if (!(std::isfinite(x) && std::isfinite(y))) return make4(0, 0, 0, 0);
     const float x0 = std::floor(x), y0 = std::floor(y);
     const float fx = x - x0, fy = y - y0;
-    const int ix0 = wrapi((int)x0, W), iy0 = wrapi((int)y0, H);
+    // beyond the int range the floored coordinate saturates, as on the device; a coordinate that is not finite makes fx or fy
+    // NaN and the blend NaN (vqcuda.h, VqSurfaceInputs)
+    const int ix0 = wrapi(to_int_sat(x0), W), iy0 = wrapi(to_int_sat(y0), H);
     const int ix1 = wrapi(ix0 + 1, W), iy1 = wrapi(iy0 + 1, H);
     const float4 t00 = ld8(base + 4 * ((size_t)iy0 * W + ix0));
     const float4 t10 = ld8(base + 4 * ((size_t)iy0 * W + ix1));

@@ -156,6 +156,8 @@ __device__ __forceinline__ void level_taps(int W, int H, uint32_t o, float u, fl
     // two roundings, as the oracle writes it: the weights multiply full-contrast byte data, so the coordinate must match
     const float x = __fsub_rn(__fmul_rn(u, (float)W), 0.5f), y = __fsub_rn(__fmul_rn(v, (float)H), 0.5f);
     const float x0 = floorf(x), y0 = floorf(y);
+    // (int) is cvt.rzi: NaN -> 0 and saturated beyond the int range, which the oracle spells out. A coordinate that is not
+    // finite gives fx or fy = NaN, so that level's blend is NaN (vqcuda.h, VqSurfaceInputs)
     fx = __fsub_rn(x, x0); fy = __fsub_rn(y, y0);
     const bool pow2 = ((W & (W - 1)) | (H & (H - 1))) == 0;
     int ix0, iy0;
@@ -454,7 +456,7 @@ __device__ __forceinline__ void shade_surface_pixel(const SurfArgs& A, int x, in
     float3 Nout = N;
     if (S.nrm) {
         const float* s = S.n;
-        if (sqrtf(s[0] * s[0] + s[1] * s[1] + s[2] * s[2]) >= 0.01f) {
+        if (!(sqrtf(s[0] * s[0] + s[1] * s[1] + s[2] * s[2]) < 0.01f)) {                          // :267 as written: NaN unpacks
             const float3 T0 = Tw * rsqrtf(dot(Tw, Tw));
             float3 sn = f3(s[0] * 2.0f - 1.0f, s[1] * 2.0f - 1.0f, s[2] * 2.0f - 1.0f);               // ShadingMath.hlsl:46
             sn = sn * rsqrtf(dot(sn, sn));
@@ -562,6 +564,11 @@ extern "C" int vq_material_table_create(VqContext* ctx, const VqMaterialData* ma
     DevMaterial* host = (DevMaterial*)calloc((size_t)count, sizeof(DevMaterial));
     if (!host) { vq_set_error("out of host memory"); return VQ_ERR_OUT_OF_MEMORY; }
     for (int i = 0; i < count; ++i) {
+        // the kernel converts textureConfig with (int): defined, and the same on host and device, only inside [0, 2^31)
+        const float cfg = materials[i].textureConfig;
+        if (!(cfg >= 0.0f && cfg < 2147483648.0f)) {
+            free(host); vq_set_error("invalid argument: material %d textureConfig %g outside [0, 2^31)", i, (double)cfg); return VQ_ERR_INVALID_ARG;
+        }
         host[i].c = materials[i];
         const VqTexture2D* src = &textures[i].diffuse;     // 7 consecutive descriptors
         for (int k = 0; k < 7; ++k) {
