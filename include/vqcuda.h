@@ -135,6 +135,14 @@ typedef struct VqPeerSignal {
  *     This entry point binds no shadow maps: caster lists and a shadowing directional light are lit with shadow
  *     factor 1 (no occlusion) - which differs from PSMain whenever the engine has shadow maps bound; use
  *     vq_forward_lighting_shadowed (below) for the PCF-shadowed result.
+ *     Where the shader text leaves the result undefined, K1 defines it (DESIGN.md §5):
+ *       - a spot cosine that rounds outside [-1, 1] (on the spot's axis, or directly behind it) is clamped, so the pixel gets
+ *         the on-axis (or opposite) intensity; HLSL's acos is unspecified there and the reference C++ gives NaN;
+ *       - a pixel exactly at a point or spot light's position (squared distance 0) gets nothing from that light (its
+ *         direction is undefined); the reference divides 0 by 0;
+ *       - closer than 1e-13 to a light (squared distance < 1e-26) the light vector is scaled by 1/sqrt(d2 + 1e-30), so the
+ *         light is dimmer than 1/d2 and stays finite where the reference overflows;
+ *       - a pixel exactly at the camera position has no view direction and shades to NaN.
  * ------------------------------------------------------------------------------------------ */
 VQ_API int vq_forward_lighting(VqContext* ctx,
                                const VqPerFrameData* per_frame,

@@ -41,7 +41,7 @@ struct F8 { float4 a, b; };
 
 struct SPoint { float3 pos; float d2Limit; float3 color; float brightness; };
 struct SDir { float3 wi; float pad0; float3 radiance; float pad1; };
-struct SSpot { float3 pos; float outer; float3 color; float brightness; float3 dir; float inner; float invCone; float pad[3]; };
+struct SSpot { float3 pos; float outer; float3 color; float brightness; float3 dir; float inner; float invCone; float cosLo, cosHi; float pad; };
 constexpr int FWD_MAX_POINT = VQ_NUM_LIGHTS_POINT + VQ_NUM_SHADOWING_LIGHTS_POINT, FWD_MAX_SPOT = VQ_NUM_LIGHTS_SPOT + VQ_NUM_SHADOWING_LIGHTS_SPOT;
 
 struct FwdParams {
@@ -242,6 +242,18 @@ __device__ __noinline__ float exact_nv(float3 cam, float3 P, uint32_t nrmTexel) 
     return dot_u(N, Wo);
 }
 
+// ---- exact re-evaluation of a spot's cosine near its axis ------------------------------------------------------------
+// SpotlightIntensity (Lighting.hlsl:57-73) takes acos of dot(normalize(P - Lpos), spotDir). Near the axis dtheta = dcos / sin(theta),
+// so the few ulp by which the fast cosine (rsqrt.approx, FMA contraction) differs from the oracle's move theta by up to 5e-4 rad there,
+// and the ramp multiplies that by 1/(outer - inner). Where that product can exceed 2^-5 * (cosine difference) / sin(theta), i.e. for
+// sin(theta) < 2^-5 * invCone, and theta can lie on the ramp, the kernel recomputes the cosine with the oracle's operation sequence.
+// The band [cosLo, cosHi] of cosines that need it is per light (condition_lights); it is empty for cones whose ramp starts beyond
+// that angle, as in every scene of bench.py.
+__device__ __noinline__ float exact_spot_cos(float3 P, float3 lpos, float3 dir) {
+    const float3 d = f3(__fsub_rn(P.x, lpos.x), __fsub_rn(P.y, lpos.y), __fsub_rn(P.z, lpos.z));
+    return dot_u(normalize_u(d), dir);
+}
+
 constexpr int FWD_THREADS = 128;
 constexpr int FWD_TILE = 2 * FWD_THREADS;          // pixels per tile: 256 consecutive pixels of one row (4 KB per G-buffer plane)
 constexpr uint32_t FWD_PLANE = FWD_TILE * 16u;     // bytes between the planes of one stage
@@ -254,7 +266,8 @@ constexpr uint32_t FWD_PLANE = FWD_TILE * 16u;     // bytes between the planes o
 // H.V = (1+c)*rh with rh = rsqrt(2+2c).
 // The body is branch-free (a light that does not contribute gets weight 0); only the rare exact-N.H slow path branches.
 // TINY: the `denom < EPSILON -> D = 1` escape of NormalDistributionGGX (BRDF.hlsl:77) can only trigger when
-// PI*(1+min(a2-1,0))^2 < 1e-12, i.e. roughness < 0.024: the caller picks the instantiation per warp, so ordinary
+// PI*(1+min(a2-1,0))^2 < 1e-12, i.e. roughness < (1e-12/PI)^(1/8) = 0.0274 (in fp32 at N.H = 1: t = (a2-1)+1 is a multiple
+// of 2^-24 and the escape holds up to t = 9*2^-24); the caller votes with 2e-12 (roughness < 0.0298) and picks the instantiation per warp, so ordinary
 // materials never pay for the selects.
 template <bool TINY>
 __device__ __forceinline__ void shade_light2(const Px2& s, Acc2& acc, float3 cam, f2 Lx, f2 Ly, f2 Lz, f2 d2, f2 invD,
@@ -342,10 +355,16 @@ __device__ __forceinline__ void shade_all_lights(const Px2& s, Acc2& acc, const 
         const SSpot l = P.spots[k];
         const LightVec2 L = light_vector2(s, l.pos);
         const f2 cosT = dot3(L.x, L.y, L.z, bc(l.dir.x), bc(l.dir.y), bc(l.dir.z)) * L.invD;   // pixel direction = -Wi
+        float cq[2] = {-cosT.v.x, -cosT.v.y};
+        if (l.cosLo < 1.5f) {                                            // warp-uniform: most cones have no exact band
+            if (cq[0] > l.cosLo && cq[0] < l.cosHi) cq[0] = exact_spot_cos(s.PA, l.pos, l.dir);   // near the axis, on the ramp
+            if (cq[1] > l.cosLo && cq[1] < l.cosHi) cq[1] = exact_spot_cos(s.PB, l.pos, l.dir);
+        }
         float inten[2];
 #pragma unroll
         for (int q = 0; q < 2; ++q) {
-            const float theta = acosf(fminf(fmaxf(-(q ? cosT.v.y : cosT.v.x), -1.0f), 1.0f));
+            // clamped: a cosine that rounds outside [-1, 1] gives the on-axis (or opposite) angle, where the reference's acos is NaN
+            const float theta = acosf(fminf(fmaxf(cq[q], -1.0f), 1.0f));
             const float lin = 1.0f - (theta - l.inner) * l.invCone;
             inten[q] = theta > l.outer ? 0.0f : (theta <= l.inner ? 1.0f : lin);
         }
@@ -866,6 +885,18 @@ static void condition_lights(const VqSceneLighting& L, FwdParams& P) {
         s.dir = make_float3(n[0], n[1], n[2]);
         s.outer = l.outerConeAngle; s.inner = l.innerConeAngle;
         s.invCone = 1.0f / (l.outerConeAngle - l.innerConeAngle);
+        // the band of cosines recomputed exactly (exact_spot_cos): theta in [inner, min(asin(2^-5 * invCone), outer)], widened by
+        // 2e-6 on both sides (more than the fast cosine's error); empty (cosLo = 2) when the ramp is unreachable or starts beyond it
+        const double ic = 1.0 / ((double)l.outerConeAngle - (double)l.innerConeAngle);
+        s.cosLo = 2.0f; s.cosHi = 2.0f;
+        if (ic > 0.0) {
+            const double thB = ic * 0x1p-5 >= 1.0 ? 1.5707963267948966 : asin(ic * 0x1p-5);
+            const double thX = fmin(thB, (double)l.outerConeAngle);
+            if (thX >= (double)l.innerConeAngle) {
+                s.cosLo = (float)(cos(thX) - 2e-6);
+                s.cosHi = l.innerConeAngle > 0.0f ? (float)(cos((double)l.innerConeAngle) + 2e-6) : 2.0f;
+            }
+        }
     }
     P.dirEnabled = L.directional.enabled != 0;
     if (P.dirEnabled) {
