@@ -77,19 +77,18 @@ struct FwdParams {
 // ---------------------------------------------------------------------------------------------
 // D3D face selection (largest |component|; ties X > Y > Z as in the oracle) written with selects so that a warp never
 // diverges on it:  face, and the face-plane coordinates sx (right), sy (up) in [-1,1]
+//   +X: (-z, y)  -X: (z, y)  +Y: (x, -z)  -Y: (x, z)  +Z: (x, y)  -Z: (-x, y), each over |major|
+// The sign choices ride on the SIGNED reciprocal of the major component: rcp.approx is odd, so (+-c) * rcp(|m|) ==
+// c' * rcp(m) bit for bit with c' = -z on X and Y, x on Z (a zero or NaN product is the same zero or NaN downstream).
 __device__ __forceinline__ void dir_to_face(float3 d, int& face, float& sx, float& sy) {
     const float ax = fabsf(d.x), ay = fabsf(d.y), az = fabsf(d.z);
     const bool isX = ax >= ay && ax >= az;
     const bool isY = !isX && ay >= az;
-    const float ma = isX ? ax : (isY ? ay : az);
     const float mv = isX ? d.x : (isY ? d.y : d.z);          // signed major component
-    const bool pos = mv > 0.0f;
-    const float r = rcp_fast(ma);
-    // +X: (-z, y)  -X: (z, y)  +Y: (x, -z)  -Y: (x, z)  +Z: (x, y)  -Z: (-x, y)
-    const float u = isX ? (pos ? -d.z : d.z) : (isY ? d.x : (pos ? d.x : -d.x));
-    const float v = isY ? (pos ? -d.z : d.z) : d.y;
-    sx = u * r; sy = v * r;
-    face = (isX ? 0 : (isY ? 2 : 4)) + (pos ? 0 : 1);
+    const float r = rcp_fast(mv), ra = fabsf(r);             // rcp(|mv|) == |rcp(mv)|
+    sx = (isX ? -d.z : d.x) * (isY ? ra : r);
+    sy = (isY ? -d.z : d.y) * (isY ? r : ra);
+    face = (isX ? 0 : (isY ? 2 : 4)) + (mv > 0.0f ? 0 : 1);
 }
 
 // integer-only neighbour lookup for a tap one texel outside the face (see DESIGN.md "cube edges"); used only by
@@ -197,22 +196,34 @@ __device__ __noinline__ float3 normalize_u_generic(float3 v) {
     const float l = __fsqrt_rn(dot_u(v, v));
     return f3(__fdiv_rn(v.x, l), __fdiv_rn(v.y, l), __fdiv_rn(v.z, l));
 }
-__device__ __forceinline__ float3 normalize_u(float3 v) {
-    const float d = dot_u(v, v);
-    if (!len2_inrange(d)) return normalize_u_generic(v);                          // never taken for sane geometry
+__device__ __forceinline__ float3 normalize_inrange(float3 v, float d) {
     const RcpRn r = rcp_rn_prepare(sqrt_rn_inrange(d));
     return f3(div_rn_inrange(v.x, r), div_rn_inrange(v.y, r), div_rn_inrange(v.z, r));
 }
+__device__ __forceinline__ float3 normalize_u(float3 v) {
+    const float d = dot_u(v, v);
+    if (!len2_inrange(d)) return normalize_u_generic(v);                          // never taken for sane geometry
+    return normalize_inrange(v, d);
+}
+// normalize_u of the result of a normalize_u: that is a unit vector (|v|^2 within a few ulp of 1), or a zero vector or one
+// with NaN components (zero or non-finite sources), which both sequences turn into all-NaN: no range check needed
+__device__ __forceinline__ float3 renormalize_u(float3 v) { return normalize_inrange(v, dot_u(v, v)); }
 
-// nrmTexel: the pixel's raw {N.xyz, roughness} texel in the shared-memory stage (still valid: the stage is released
-// after the pixel is finished)
-__device__ __noinline__ float exact_ndoth(float3 cam, float3 P, uint32_t nrmTexel, float3 wiSrc, float wiLenSq) {
-    float4 nr;
-    asm volatile("ld.shared.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(nr.x), "=f"(nr.y), "=f"(nr.z), "=f"(nr.w) : "r"(nrmTexel));
+constexpr int FWD_THREADS = 128;
+constexpr int FWD_TILE = 2 * FWD_THREADS;          // pixels per tile: 256 consecutive pixels of one row (4 KB per G-buffer plane)
+constexpr uint32_t FWD_PLANE = FWD_TILE * 16u;     // bytes between the planes of one stage
+
+// posTexel: the pixel's position texel in the shared-memory stage, its raw {N.xyz, roughness} texel one plane further (still
+// valid: the stage is released after the pixel is finished). Reading P there rather than taking it as arguments keeps the
+// call sites in the light loop short.
+__device__ __noinline__ float exact_ndoth(float3 cam, uint32_t posTexel, float3 wiSrc, float wiLenSq) {
+    float4 pa, nr;
+    asm volatile("ld.shared.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(pa.x), "=f"(pa.y), "=f"(pa.z), "=f"(pa.w) : "r"(posTexel));
+    asm volatile("ld.shared.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(nr.x), "=f"(nr.y), "=f"(nr.z), "=f"(nr.w) : "r"(posTexel + FWD_PLANE));
     const float3 Ns = f3(nr.x, nr.y, nr.z);
-    const float3 Vv = f3(__fsub_rn(cam.x, P.x), __fsub_rn(cam.y, P.y), __fsub_rn(cam.z, P.z));
+    const float3 Vv = f3(__fsub_rn(cam.x, pa.x), __fsub_rn(cam.y, pa.y), __fsub_rn(cam.z, pa.z));
     const float3 V = normalize_u(Vv);                 // ForwardLighting.hlsl:285
-    const float3 Wo = normalize_u(V);                 // BRDF.hlsl:166
+    const float3 Wo = renormalize_u(V);               // BRDF.hlsl:166
     const float3 N = normalize_u(Ns);                 // BRDF.hlsl:167
     float3 Wi;                                        // Lighting.hlsl:312: Lv / length(Lv)
     if (len2_inrange(wiLenSq)) {
@@ -237,7 +248,7 @@ __device__ __noinline__ float exact_nv(float3 cam, float3 P, uint32_t nrmTexel) 
     float4 nr;
     asm volatile("ld.shared.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(nr.x), "=f"(nr.y), "=f"(nr.z), "=f"(nr.w) : "r"(nrmTexel));
     const float3 Vv = f3(__fsub_rn(cam.x, P.x), __fsub_rn(cam.y, P.y), __fsub_rn(cam.z, P.z));
-    const float3 Wo = normalize_u(normalize_u(Vv));                 // ForwardLighting.hlsl:285, BRDF.hlsl:166
+    const float3 Wo = renormalize_u(normalize_u(Vv));               // ForwardLighting.hlsl:285, BRDF.hlsl:166
     const float3 N = normalize_u(f3(nr.x, nr.y, nr.z));             // BRDF.hlsl:167
     return dot_u(N, Wo);
 }
@@ -253,10 +264,6 @@ __device__ __noinline__ float exact_spot_cos(float3 P, float3 lpos, float3 dir) 
     const float3 d = f3(__fsub_rn(P.x, lpos.x), __fsub_rn(P.y, lpos.y), __fsub_rn(P.z, lpos.z));
     return dot_u(normalize_u(d), dir);
 }
-
-constexpr int FWD_THREADS = 128;
-constexpr int FWD_TILE = 2 * FWD_THREADS;          // pixels per tile: 256 consecutive pixels of one row (4 KB per G-buffer plane)
-constexpr uint32_t FWD_PLANE = FWD_TILE * 16u;     // bytes between the planes of one stage
 
 // One light for the pixel pair: accumulates BRDF(s, Wi, V) * radiance * NdotL (BRDF.hlsl:163-194, Lighting.hlsl:308-345) in the
 // factored form  r = K1*(1-fc) + omF0*(fc*spec) + F0*spec  with  F = F0 + (1-F0)*fc.
@@ -285,11 +292,11 @@ __device__ __forceinline__ void shade_light2(const Px2& s, Acc2& acc, float3 cam
     const f2 w = mulsat2(s.nsLen, nl) * scale;            // NdotL of the raw s.N (Lighting.hlsl:316) * radiance scale
     if (fminf(t.v.x, t.v.y) < T_EXACT) {                  // < 1 % of pixel-light pairs
         if (t.v.x < T_EXACT && w.v.x > 0.0f) {
-            const float nh = exact_ndoth(cam, s.PA, s.texA + FWD_PLANE, f3(Lx.v.x, Ly.v.x, Lz.v.x), d2.v.x);
+            const float nh = exact_ndoth(cam, s.texA, f3(Lx.v.x, Ly.v.x, Lz.v.x), d2.v.x);
             t.v.x = __fadd_rn(__fmul_rn(__fmul_rn(nh, nh), s.a2m1.v.x), 1.0f);
         }
         if (t.v.y < T_EXACT && w.v.y > 0.0f) {
-            const float nh = exact_ndoth(cam, s.PB, s.texB + FWD_PLANE, f3(Lx.v.y, Ly.v.y, Lz.v.y), d2.v.y);
+            const float nh = exact_ndoth(cam, s.texB, f3(Lx.v.y, Ly.v.y, Lz.v.y), d2.v.y);
             t.v.y = __fadd_rn(__fmul_rn(__fmul_rn(nh, nh), s.a2m1.v.y), 1.0f);
         }
     }
@@ -512,9 +519,13 @@ __device__ __forceinline__ CubeLoad cube_issue(const float4* __restrict__ texels
     const uint32_t off = min(f.base + (uint32_t)((int)yf + 1) * f.P + (uint32_t)((int)xf + 1), maxRec);
     uint32_t e0, o0, e1, o1;
     pair_halves(off, e0, o0);
-    if (UNIFORM_P) { e1 = e0 + f.P; o1 = o0 + f.P; }
-    else pair_halves(off + f.P, e1, o1);
-    L.r0 = ldg_pair(texels, e0, o0); L.r1 = ldg_pair(texels, e1, o1);
+    L.r0 = ldg_pair(texels, e0, o0);
+    if (UNIFORM_P) {                                          // the second row from a row-shifted base: no per-lane adds
+        L.r1 = ldg_pair(texels + f.P, e0, o0);
+    } else {
+        pair_halves(off + f.P, e1, o1);
+        L.r1 = ldg_pair(texels, e1, o1);
+    }
     return L;
 }
 // bilinear blend of the footprint as pairs {x,y}, {z,w} of one pixel
