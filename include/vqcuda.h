@@ -385,6 +385,23 @@ VQ_API int vq_gbuffer_from_materials(VqContext* ctx, const VqSurfaceInputs* in, 
                                      float ambient_factor, int alpha_mask, const VqGBuffer* out,
                                      int row_begin, int row_end, void* stream);
 
+/* PSMain end to end (ForwardLighting.hlsl:222-391) in ONE launch, from interpolants and materials to lit colour: computes
+ * what vq_gbuffer_from_materials(ctx, in, table, per_frame->fAmbientLightingFactor, alpha_mask, &gb, ...) with an emissive
+ * plane, followed by vq_forward_lighting(ctx, per_frame, per_view, &gb, env, out_color, ...), computes, bit for bit (with a
+ * non-zero fHDRIOffsetInRadians a few pixels may differ in their last bits: the compiler contracts the yaw rotation of the
+ * cube lookups differently in the two kernels), but the G-buffer never leaves the SM (no device memory is allocated or written for it). out_color has the size of the attribute
+ * planes and receives {I.rgb, roughness}. Pixels the alpha mask discards are left untouched in out_color, as a discarded
+ * fragment writes nothing. Rows [row_begin,row_end) follow vq_gbuffer_from_materials: quads are aligned to absolute even rows,
+ * so row ranges tile the image. The defined deviations from the shader text are those of the two halves: the sampling rules
+ * of vq_gbuffer_from_materials / VqSurfaceInputs and the K1 list at vq_forward_lighting. No shadow maps are bound (lit as
+ * vq_forward_lighting lights them): the PCF pre-pass of vq_forward_lighting_shadowed needs the world position of every pixel
+ * in device memory, which is the G-buffer this call does without. The arguments are checked before the device is touched.
+ * Like vq_forward_lighting, it rebuilds the IBL sampling copies per call unless the environment is registered. */
+VQ_API int vq_forward_lighting_from_materials(VqContext* ctx, const VqPerFrameData* per_frame,
+                                              const VqPerViewLightingData* per_view, const VqSurfaceInputs* in,
+                                              const VqMaterialTable* table, int alpha_mask, const VqEnvironmentMaps* env,
+                                              VqImage out_color, int row_begin, int row_end, void* stream);
+
 /* ------------------------------------------------------------------------------------------
  * SURVEY §8(f).2  On-disk format at either end of the path: Radiance .hdr (RGBE).
  *     Load  = Image::LoadFromFile -> stbi_loadf(path, &x, &y, &n, 4) (Libs/VQUtils/Source/Image.cpp:119-121) with

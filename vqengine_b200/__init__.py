@@ -34,6 +34,7 @@ ABI_SYMBOLS = [
     "vq_hdr_parse", "vq_hdr_decode", "vq_hdr_load_host", "vq_hdr_encode_rgbe", "vq_hdr_pack_file", "vq_hdr_save_host",
     "vq_skydome", "vq_apply_reflections", "vq_specular_prefilter_multi", "vq_specular_prefilter_ranges", "vq_forward_lighting_multi_signal", "vq_image_resize", "vq_resize_axis_table",
     "vq_forward_lighting_shadowed", "vq_depth_pyramid_level_count", "vq_depth_pyramid_texel_count", "vq_depth_min_pyramid",
+    "vq_forward_lighting_from_materials",
 ]
 
 
@@ -102,6 +103,8 @@ def _load() -> C.CDLL:
     lib.vq_material_table_create.argtypes = [vp, P(MaterialData), P(MaterialTextures), C.c_int, P(vp)]
     lib.vq_material_table_destroy.argtypes = [vp, vp]
     lib.vq_gbuffer_from_materials.argtypes = [vp, P(SurfaceInputs), vp, f32, C.c_int, P(GBuffer), C.c_int, C.c_int, vp]
+    lib.vq_forward_lighting_from_materials.argtypes = [vp, P(PerFrameData), P(PerViewLightingData), P(SurfaceInputs), vp, C.c_int,
+                                                       P(EnvironmentMaps), Image, C.c_int, C.c_int, vp]
     u64 = C.c_uint64
     lib.vq_hdr_parse.argtypes = [vp, u64, P(HdrInfo), P(u64)]
     lib.vq_hdr_decode.argtypes = [vp, vp, u64, P(HdrInfo), vp, Image, vp, vp]
@@ -358,6 +361,14 @@ class Context:
         _check(lib.vq_gbuffer_from_materials(self._h, C.byref(inputs), table._h, ambient_factor, 1 if alpha_mask else 0,
                                              C.byref(gbuffer), row_begin, h if row_end is None else row_end,
                                              _stream_ptr(stream)))
+
+    def forward_lighting_from_materials(self, per_frame, per_view, inputs: SurfaceInputs, table: "MaterialTable", env: EnvironmentMaps,
+                                        out, alpha_mask: bool = False, row_begin=0, row_end=None, stream=None):
+        """PSMain end to end in one launch: gbuffer_from_materials (with emissive) + forward_lighting, no G-buffer"""
+        h = inputs.position_u.height
+        _check(lib.vq_forward_lighting_from_materials(self._h, C.byref(per_frame), C.byref(per_view), C.byref(inputs), table._h,
+                                                      1 if alpha_mask else 0, C.byref(env), image_of(out), row_begin,
+                                                      h if row_end is None else row_end, _stream_ptr(stream)))
 
     # SURVEY 8(f).2: Radiance .hdr
     def hdr_decode(self, file_bytes: bytes, stream=None):

@@ -16,6 +16,7 @@
 //   * the specular mip is int(roughness * MAX_LOD) (one fp32 multiply);
 //   * cubemap taps are seamless across face edges, so face selection is not a discontinuity.
 #include "vq_common.cuh"
+#include "vq_surface_sample.cuh"
 #include <stdlib.h>
 
 using namespace vq;
@@ -626,10 +627,10 @@ __device__ __forceinline__ float4 compose_pixel(const FwdParams& P, uint32_t tex
     return compose_values(P, texel, nsnv, roughness, ao, la, lb, lc, diffIrr, specCol, sb);
 }
 
-// everything after the light loop for the pixel pair: environment taps, composition, stores
+// everything after the light loop for the pixel pair: environment taps, composition, stores (pixel A to (yA, xA), B to (yB, xB))
 template <bool MULTI, bool ROT, bool SPEC>
 __device__ __forceinline__ void finish_pair(const FwdParams& P, const FaceRec* __restrict__ sFace, const Px2& s, const Acc2& acc, f2 roughness, f2 ao,
-                                            int y, int xA, int xB, bool validA, bool validB) {
+                                            int yA, int xA, int yB, int xB, bool validA, bool validB) {
     const f2 nsnv = mulsat2(s.nsLen, s.nv);                      // saturate(dot(s.N, V)) of the raw normal
     const f2 Nrx = s.Nx * s.nsLen, Nry = s.Ny * s.nsLen, Nrz = s.Nz * s.nsLen;
     EnvLoads eA, eB;
@@ -638,14 +639,14 @@ __device__ __forceinline__ void finish_pair(const FwdParams& P, const FaceRec* _
     const float4 oA = compose_pixel<SPEC>(P, s.texA, nsnv.v.x, roughness.v.x, ao.v.x, f3(acc.ax.v.x, acc.ay.v.x, acc.az.v.x),
                                           f3(acc.bx.v.x, acc.by.v.x, acc.bz.v.x), f3(acc.cx.v.x, acc.cy.v.x, acc.cz.v.x), eA);
     if (validA) {   // one STG.128 per destination; peer destinations are mapped NVLink addresses (fused compute + gather)
-        if (MULTI) { for (int q = 0; q < P.nOut; ++q) st_stream(P.outs[q].row(P.dstRowOffset + y) + xA, oA); }
-        else st_stream_hint(P.outs[0].row(P.dstRowOffset + y) + xA, oA, l2_evict_first_policy());
+        if (MULTI) { for (int q = 0; q < P.nOut; ++q) st_stream(P.outs[q].row(P.dstRowOffset + yA) + xA, oA); }
+        else st_stream_hint(P.outs[0].row(P.dstRowOffset + yA) + xA, oA, l2_evict_first_policy());
     }
     const float4 oB = compose_pixel<SPEC>(P, s.texB, nsnv.v.y, roughness.v.y, ao.v.y, f3(acc.ax.v.y, acc.ay.v.y, acc.az.v.y),
                                           f3(acc.bx.v.y, acc.by.v.y, acc.bz.v.y), f3(acc.cx.v.y, acc.cy.v.y, acc.cz.v.y), eB);
     if (validB) {
-        if (MULTI) { for (int q = 0; q < P.nOut; ++q) st_stream(P.outs[q].row(P.dstRowOffset + y) + xB, oB); }
-        else st_stream_hint(P.outs[0].row(P.dstRowOffset + y) + xB, oB, l2_evict_first_policy());
+        if (MULTI) { for (int q = 0; q < P.nOut; ++q) st_stream(P.outs[q].row(P.dstRowOffset + yB) + xB, oB); }
+        else st_stream_hint(P.outs[0].row(P.dstRowOffset + yB) + xB, oB, l2_evict_first_policy());
     }
 }
 
@@ -692,6 +693,20 @@ __device__ __forceinline__ void shade_pair_lights(const FwdParams& P, Px2& s, Ac
         shade_all_lights<false, SHADOWED>(s, acc, P);
 }
 
+// entry i = face*16 + mip of the specular cube's face table, staged once per CTA: the lanes of a warp mostly share the face and
+// differ in the mip (per-pixel roughness), so the entries they read are ADJACENT 16-byte words in different banks (mip*8+face
+// measured 19 wavefronts per LDS.128, ideal 4)
+__device__ __forceinline__ FaceRec face_rec(const FwdParams& P, int i) {
+    const int mip = i & 15, face = i >> 4;
+    FaceRec f; f.base = 0u; f.P = 3u; f.halfN = 0.5f; f.c0 = 0.0f;
+    if (!P.diffuseOnly && mip < P.spec.mips && face < 6) {
+        const int N = P.spec.res >> mip;
+        f.P = (uint32_t)N + 2u; f.base = P.spec.mipOffset[mip] + (uint32_t)face * f.P * f.P;
+        f.halfN = 0.5f * (float)N; f.c0 = f.halfN - 0.5f;
+    }
+    return f;
+}
+
 template <bool MULTI, bool ROT, bool SHADOWED = false>
 __global__ void __launch_bounds__(FWD_THREADS, FWD_CTAS_PER_SM) forward_kernel(const __grid_constant__ FwdParams P) {
     extern __shared__ __align__(128) unsigned char smemRaw[];
@@ -730,19 +745,7 @@ __global__ void __launch_bounds__(FWD_THREADS, FWD_CTAS_PER_SM) forward_kernel(c
         for (int s = 0; s < FWD_AHEAD; ++s) request((int)blockIdx.y + s * rowStep, s, 0u);   // prologue: FWD_AHEAD tiles in flight
     }
 
-    // ---- stage the specular cube's face table, once per CTA ----
-    for (int i = tid; i < 16 * 8; i += FWD_THREADS) {
-        // index = face*16 + mip: the lanes of a warp mostly share the face and differ in the mip (per-pixel roughness), so the
-        // entries they read are ADJACENT 16-byte words in different banks (mip*8+face measured 19 wavefronts per LDS.128, ideal 4)
-        const int mip = i & 15, face = i >> 4;
-        FaceRec f; f.base = 0u; f.P = 3u; f.halfN = 0.5f; f.c0 = 0.0f;
-        if (!P.diffuseOnly && mip < P.spec.mips && face < 6) {
-            const int N = P.spec.res >> mip;
-            f.P = (uint32_t)N + 2u; f.base = P.spec.mipOffset[mip] + (uint32_t)face * f.P * f.P;
-            f.halfN = 0.5f * (float)N; f.c0 = f.halfN - 0.5f;
-        }
-        sFace[i] = f;
-    }
+    for (int i = tid; i < 16 * 8; i += FWD_THREADS) sFace[i] = face_rec(P, i);     // the specular cube's face table
     __syncthreads();                                              // face table staged, mbarriers initialised
 
     int st = 0; uint32_t use = 0;                                 // stage of the current tile, completed uses of that stage
@@ -770,8 +773,8 @@ __global__ void __launch_bounds__(FWD_THREADS, FWD_CTAS_PER_SM) forward_kernel(c
                 s.recA = ((uint64_t)ra.y << 32) | ra.x; s.recB = ((uint64_t)rb.y << 32) | rb.x;
             }
             shade_pair_lights<SHADOWED>(P, s, acc, roughness, ao);
-            if (P.diffuseOnly) finish_pair<MULTI, ROT, false>(P, sFace, s, acc, roughness, ao, y, xA, xB, validA, validB);
-            else finish_pair<MULTI, ROT, true>(P, sFace, s, acc, roughness, ao, y, xA, xB, validA, validB);
+            if (P.diffuseOnly) finish_pair<MULTI, ROT, false>(P, sFace, s, acc, roughness, ao, y, xA, y, xB, validA, validB);
+            else finish_pair<MULTI, ROT, true>(P, sFace, s, acc, roughness, ao, y, xA, y, xB, validA, validB);
         }
         mbar_arrive(emptyBar(st));                               // this thread is done with the stage
         if (++st == FWD_STAGES) { st = 0; ++use; }
@@ -787,6 +790,74 @@ __global__ void __launch_bounds__(FWD_THREADS, FWD_CTAS_PER_SM) forward_kernel(c
                 peer_rendezvous(P.sync);
             }
         }
+    }
+}
+
+// ---------------------------------------------------------------------------------------------
+// PSMain end to end: the surface producer and K1 fused, with the G-buffer in shared memory instead of HBM
+// ---------------------------------------------------------------------------------------------
+struct PsParams {
+    FwdParams F;                       // K1's frame (outs[0] = the destination; no G-buffer planes, no shadow records)
+    SurfArgs S;                        // the surface producer's inputs (no G-buffer outputs)
+};
+__device__ __forceinline__ void sts128(uint32_t addr, float4 v) {
+    asm volatile("st.shared.v4.f32 [%0], {%1,%2,%3,%4};" :: "r"(addr), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w) : "memory");
+}
+
+// A persistent CTA walks tiles of 2 rows x FWD_THREADS columns (rows aligned to absolute even rows, as the surface producer's
+// quads are), keeping its column and striding the row pairs by gridDim.y. Per tile, two phases separated by CTA barriers:
+//   producer: warp w runs the surface producer's per-pixel code for the 16x2 strips w and w+4 of the tile and writes the four
+//             G-buffer texels of each pixel into a shared-memory stage with K1's layout (plane k of stage pixel p at
+//             k*FWD_PLANE + 16p; row 0 of the tile is stage pixels 0..127, row 1 is 128..255), plus a flag saying whether the
+//             pixel was produced (inside the image and the row range, not discarded by the alpha mask);
+//   shading:  thread t shades the pixel pair (row 0, column t), (row 1, column t) with K1's code on the stage and stores the
+//             pixels that were produced. The lane-pair gathers pair neighbouring columns of one row, as in K1.
+// The phases stay sequential: a warp-specialised K1 measured slower (DESIGN.md §4).
+template <bool ROT>
+__global__ void __launch_bounds__(FWD_THREADS, FWD_CTAS_PER_SM) psmain_kernel(const __grid_constant__ PsParams Q) {
+    const FwdParams& P = Q.F;
+    const SurfArgs& A = Q.S;
+    __shared__ __align__(128) float4 sStage[4 * FWD_TILE];
+    __shared__ FaceRec sFace[16 * 8];
+    __shared__ uint8_t sProduced[FWD_TILE];
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const uint32_t stage0 = smem_u32(sStage);
+    // the stage starts zeroed: a pixel that is not produced is still shaded (whole warps take part in the votes and exchanges)
+    // but never stored, and it reads defined values
+    for (int i = tid; i < 4 * FWD_TILE; i += FWD_THREADS) sStage[i] = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+    for (int i = tid; i < 16 * 8; i += FWD_THREADS) sFace[i] = face_rec(P, i);
+    const int x0 = (int)blockIdx.x * FWD_THREADS;
+    const int xA = x0 + tid;
+    const bool inRow = xA < P.width;
+    const int pairs = (A.rowEnd - A.tileY0 + 1) / 2;
+    for (int t = (int)blockIdx.y; t < pairs; t += (int)gridDim.y) {
+        const int y0 = A.tileY0 + 2 * t;
+        __syncthreads();                                          // the previous tile's shading is done with the stage
+#pragma unroll 1
+        for (int k = 0; k < 2; ++k) {
+            const int c = (warp + 4 * k) * 16 + (lane & 15), r = lane >> 4;
+            const uint32_t px = (uint32_t)(r * FWD_THREADS + c);
+            bool produced = false;
+            surface_quad_pixel(A, x0 + c, y0 + r, lane, l2_policy_evict_first(), [&](float4 posAo, float4 nrmRough, float4 albMetal, float4 emi) {
+                const uint32_t texel = stage0 + px * 16u;
+                sts128(texel, posAo);
+                sts128(texel + FWD_PLANE, nrmRough);
+                sts128(texel + 2u * FWD_PLANE, albMetal);
+                sts128(texel + 3u * FWD_PLANE, emi);
+                produced = true;
+            });
+            sProduced[px] = produced ? 1 : 0;
+        }
+        __syncthreads();                                          // the tile is staged
+        Px2 s;
+        s.texA = stage0 + (uint32_t)(min(xA, P.width - 1) - x0) * 16u;   // a ragged tile: columns off the row alias its last pixel
+        s.texB = s.texA + FWD_THREADS * 16u;
+        f2 roughness, ao;
+        Acc2 acc;
+        shade_pair_lights<false>(P, s, acc, roughness, ao);
+        const bool validA = inRow && sProduced[tid] != 0, validB = inRow && sProduced[FWD_THREADS + tid] != 0;
+        if (P.diffuseOnly) finish_pair<false, ROT, false>(P, sFace, s, acc, roughness, ao, y0, xA, y0 + 1, xA, validA, validB);
+        else finish_pair<false, ROT, true>(P, sFace, s, acc, roughness, ao, y0, xA, y0 + 1, xA, validA, validB);
     }
 }
 
@@ -919,6 +990,45 @@ static void condition_lights(const VqSceneLighting& L, FwdParams& P) {
     }
 }
 
+static bool light_counts_ok(const VqSceneLighting& L) {
+    return L.numPointLights >= 0 && L.numPointLights <= VQ_NUM_LIGHTS_POINT && L.numSpotLights >= 0 && L.numSpotLights <= VQ_NUM_LIGHTS_SPOT &&
+           L.numPointCasters >= 0 && L.numPointCasters <= VQ_NUM_SHADOWING_LIGHTS_POINT &&
+           L.numSpotCasters >= 0 && L.numSpotCasters <= VQ_NUM_SHADOWING_LIGHTS_SPOT;
+}
+
+// What K1 reads of the frame but the surface: lights, camera, HDRI yaw, environment (its sampling copies: the registered ones
+// when they match, else built now on `stream`). Call with the context's scratch locked.
+static int frame_params(VqContext* ctx, const VqPerFrameData* pf, const VqPerViewLightingData* pv, const VqEnvironmentMaps* env,
+                        cudaStream_t stream, FwdParams& P) {
+    condition_lights(pf->Lights, P);
+    P.cam = make_float3(pv->CameraPosition.x, pv->CameraPosition.y, pv->CameraPosition.z);
+    P.cosB = cosf(-pf->fHDRIOffsetInRadians);
+    P.sinB = sinf(-pf->fHDRIOffsetInRadians);
+    P.maxLod = (int)pv->MaxEnvMapLODLevels;
+    P.diffuseOnly = pv->EnvironmentMapDiffuseOnlyIllumination != 0;
+    VQ_REQUIRE(cube_desc_ok(env->irradiance_diffuse), "bad cubemap descriptor (irradiance_diffuse)");
+    if (!P.diffuseOnly) {
+        VQ_REQUIRE(cube_desc_ok(env->irradiance_specular), "bad cubemap descriptor (irradiance_specular)");
+        VQ_REQUIRE(vq_image_ok(env->brdf_lut, 8), "bad BRDF LUT descriptor");
+        VQ_REQUIRE(env->brdf_lut.width <= 8192 && env->brdf_lut.height <= 8192, "BRDF LUT larger than 8192^2");
+        P.lut.w = env->brdf_lut.width; P.lut.h = env->brdf_lut.height;
+    }
+    // bordered sampling copies: from the prepared environment when it matches (the descriptors checked above are non-null, so
+    // a match also means the registration holds every part this call reads), else built now on this stream
+    const bool full = !P.diffuseOnly;
+    const bool prepared = ctx->env_valid && same_cube(ctx->env_key.irradiance_diffuse, env->irradiance_diffuse) &&
+                          (P.diffuseOnly || (same_cube(ctx->env_key.irradiance_specular, env->irradiance_specular) &&
+                                             same_image(ctx->env_key.brdf_lut, env->brdf_lut)));
+    if (prepared) sampling_views(*env, full, full, (uintptr_t)ctx->env_prepared.p, P.diff, P.spec, P.lut);
+    else {
+        const int rc = build_sampling_copies(ctx->env_per_call, *env, full, full, stream, P.diff, P.spec, P.lut); if (rc) return rc;
+    }
+    P.diffHalfN = 0.5f * (float)env->irradiance_diffuse.res;
+    P.diffMaxRec = (uint32_t)padded_texels(env->irradiance_diffuse.res, 1) - 1u;      // K1 samples mip 0 of the diffuse cube only
+    P.specMaxRec = P.diffuseOnly ? 0u : (uint32_t)padded_texels(env->irradiance_specular.res, env->irradiance_specular.mips) - 1u;
+    return VQ_OK;
+}
+
 int vq_forward_launch_multi(VqContext* ctx, const VqPerFrameData* pf, const VqPerViewLightingData* pv,
                             const VqGBuffer* gb, const VqEnvironmentMaps* env, const VqImage* outs, int n_outs,
                             int dst_row_offset, int row_begin, int row_end, const VqPeerSignal* sig, cudaStream_t stream,
@@ -935,22 +1045,13 @@ int vq_forward_launch_multi(VqContext* ctx, const VqPerFrameData* pf, const VqPe
                    "every destination must be as wide as the G-buffer and hold dst_row_offset + height rows");
     VQ_REQUIRE(row_begin >= 0 && row_end <= H && row_begin <= row_end, "row range out of bounds");
     const VqSceneLighting& L = pf->Lights;
-    VQ_REQUIRE(L.numPointLights >= 0 && L.numPointLights <= VQ_NUM_LIGHTS_POINT &&
-               L.numSpotLights >= 0 && L.numSpotLights <= VQ_NUM_LIGHTS_SPOT &&
-               L.numPointCasters >= 0 && L.numPointCasters <= VQ_NUM_SHADOWING_LIGHTS_POINT &&
-               L.numSpotCasters >= 0 && L.numSpotCasters <= VQ_NUM_SHADOWING_LIGHTS_SPOT, "light counts exceed the cbuffer arrays");
+    VQ_REQUIRE(light_counts_ok(L), "light counts exceed the cbuffer arrays");
     VQ_REQUIRE(row_begin < row_end || !(sig && sig->n_ranks > 1), "a rendezvous needs a non-empty row range (the kernel runs it)");
     if (row_begin == row_end) return VQ_OK;
     VqScratchLock lock(ctx);           // the registered environment and the per-call sampling copies are the context's
 
     FwdParams P;
     memset(&P, 0, sizeof(P));
-    condition_lights(L, P);
-    P.cam = make_float3(pv->CameraPosition.x, pv->CameraPosition.y, pv->CameraPosition.z);
-    P.cosB = cosf(-pf->fHDRIOffsetInRadians);
-    P.sinB = sinf(-pf->fHDRIOffsetInRadians);
-    P.maxLod = (int)pv->MaxEnvMapLODLevels;
-    P.diffuseOnly = pv->EnvironmentMapDiffuseOnlyIllumination != 0;
     P.pos = make_view(gb->position_ao); P.nrm = make_view(gb->normal_roughness); P.alb = make_view(gb->albedo_metalness);
     for (int k = 0; k < n_outs; ++k) P.outs[k] = make_view(outs[k]);
     P.nOut = n_outs; P.dstRowOffset = dst_row_offset;
@@ -959,24 +1060,7 @@ int vq_forward_launch_multi(VqContext* ctx, const VqPerFrameData* pf, const VqPe
         VQ_REQUIRE(vq_image_ok(gb->emissive) && gb->emissive.width == W && gb->emissive.height == H, "bad emissive plane");
         P.emi = make_view(gb->emissive);
     }
-    VQ_REQUIRE(cube_desc_ok(env->irradiance_diffuse), "bad cubemap descriptor (irradiance_diffuse)");
-    if (!P.diffuseOnly) {
-        VQ_REQUIRE(cube_desc_ok(env->irradiance_specular), "bad cubemap descriptor (irradiance_specular)");
-        VQ_REQUIRE(vq_image_ok(env->brdf_lut, 8), "bad BRDF LUT descriptor");
-        VQ_REQUIRE(env->brdf_lut.width <= 8192 && env->brdf_lut.height <= 8192, "BRDF LUT larger than 8192^2");
-        P.lut.w = env->brdf_lut.width; P.lut.h = env->brdf_lut.height;
-    }
-    // bordered sampling copies: from the prepared environment when it matches (the descriptors checked above are non-null, so
-    // a match also means the registration holds every part this call reads), else built now on this stream
-    int rc;
-    const bool full = !P.diffuseOnly;
-    const bool prepared = ctx->env_valid && same_cube(ctx->env_key.irradiance_diffuse, env->irradiance_diffuse) &&
-                          (P.diffuseOnly || (same_cube(ctx->env_key.irradiance_specular, env->irradiance_specular) &&
-                                             same_image(ctx->env_key.brdf_lut, env->brdf_lut)));
-    if (prepared) sampling_views(*env, full, full, (uintptr_t)ctx->env_prepared.p, P.diff, P.spec, P.lut);
-    else {
-        rc = build_sampling_copies(ctx->env_per_call, *env, full, full, stream, P.diff, P.spec, P.lut); if (rc) return rc;
-    }
+    int rc = frame_params(ctx, pf, pv, env, stream, P); if (rc) return rc;
     P.rowBegin = row_begin; P.rows = row_end - row_begin; P.width = W;
     const bool shadowed = shadow && shadow->p;
     if (shadowed) {
@@ -989,9 +1073,6 @@ int vq_forward_launch_multi(VqContext* ctx, const VqPerFrameData* pf, const VqPe
     rc = vq_fill_peer_sync(sig, &P.sync); if (rc) return rc;
     VQ_REQUIRE(P.sync.n == 0 || n_outs > 1, "a rendezvous only makes sense with peer destinations");
     P.ticket = P.sync.n > 1 ? vq_ticket_pair(ctx) : nullptr;
-    P.diffHalfN = 0.5f * (float)env->irradiance_diffuse.res;
-    P.diffMaxRec = (uint32_t)padded_texels(env->irradiance_diffuse.res, 1) - 1u;      // K1 samples mip 0 of the diffuse cube only
-    P.specMaxRec = P.diffuseOnly ? 0u : (uint32_t)padded_texels(env->irradiance_specular.res, env->irradiance_specular.mips) - 1u;
 
     // persistent grid: x = the row's 256-pixel tiles, y = row groups striding the rows
     const unsigned gx = (unsigned)((W + FWD_TILE - 1) / FWD_TILE);
@@ -1057,6 +1138,40 @@ extern "C" int vq_forward_lighting_multi_signal(VqContext* ctx, const VqPerFrame
     int rc = vq_enter(ctx); if (rc) return rc;
     VQ_MARK("RenderSceneColor");
     return vq_forward_launch_multi(ctx, pf, pv, gb, env, outs, n_outs, dst_row_offset, row_begin, row_end, signal, (cudaStream_t)stream);
+}
+
+// PSMain from interpolants and materials in one launch (psmain_kernel): what vq_gbuffer_from_materials with an emissive plane
+// followed by vq_forward_lighting computes, without the G-buffer. The arguments are checked before the device is touched.
+extern "C" int vq_forward_lighting_from_materials(VqContext* ctx, const VqPerFrameData* pf, const VqPerViewLightingData* pv,
+                                                  const VqSurfaceInputs* in, const VqMaterialTable* table, int alpha_mask,
+                                                  const VqEnvironmentMaps* env, VqImage out, int row_begin, int row_end, void* stream) {
+    VQ_REQUIRE(pf && pv && env && in, "null argument");
+    const int W = in->position_u.width, H = in->position_u.height;
+    VQ_REQUIRE(vq_image_ok(out) && out.width == W && out.height == H, "the output must have the size of the attribute planes");
+    static_assert(sizeof(PsParams) <= 32764, "kernel parameter space");
+    PsParams Q;
+    memset(&Q, 0, sizeof(Q));
+    int rc = surface_inputs(in, table, pf->fAmbientLightingFactor, alpha_mask, row_begin, row_end, Q.S); if (rc) return rc;
+    VQ_REQUIRE(light_counts_ok(pf->Lights), "light counts exceed the cbuffer arrays");
+    rc = vq_enter(ctx); if (rc) return rc;
+    VQ_MARK("RenderSceneColor");
+    if (row_begin == row_end) return VQ_OK;
+    VqScratchLock lock(ctx);           // the registered environment and the per-call sampling copies are the context's
+    FwdParams& P = Q.F;
+    rc = frame_params(ctx, pf, pv, env, (cudaStream_t)stream, P); if (rc) return rc;
+    P.hasEmissive = 1;
+    P.outs[0] = make_view(out); P.nOut = 1;
+    P.rowBegin = row_begin; P.rows = row_end - row_begin; P.width = W;
+    // persistent grid: x = the row's 128-column tiles, y = groups striding the row pairs
+    const unsigned gx = (unsigned)((W + FWD_THREADS - 1) / FWD_THREADS);
+    const unsigned pairs = (unsigned)((row_end - Q.S.tileY0 + 1) / 2);
+    unsigned gy = (unsigned)(ctx->sm_count * FWD_CTAS_PER_SM) / gx;
+    if (gy < 1) gy = 1;
+    if (gy > pairs) gy = pairs;
+    const bool rot = P.sinB != 0.0f || P.cosB != 1.0f;
+    if (rot) psmain_kernel<true><<<dim3(gx, gy), FWD_THREADS, 0, (cudaStream_t)stream>>>(Q);
+    else psmain_kernel<false><<<dim3(gx, gy), FWD_THREADS, 0, (cudaStream_t)stream>>>(Q);
+    return vq_check_launch("forward_lighting_from_materials");
 }
 
 // The IBL cubemaps and the BRDF LUT are sampled from footprint-friendly copies (see CubeV, LutV).

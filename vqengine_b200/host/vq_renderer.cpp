@@ -179,11 +179,11 @@ bool VQRenderer::PreFilterEnvironmentMap(FEnvironmentMapRenderingResources& env,
     return true;
 }
 
-bool VQRenderer::RenderSceneColor(cudaStream_t pCmd, const FSceneView& SceneView, const FPostProcessParameters& PPParams,
-                                  const VqGBuffer& GBuffer, const FEnvironmentMapRenderingResources& env,
-                                  const FGraphicsSettings& GFXSettings, bool bHDRDisplay) {
+// CopyPerFrameConstantBufferData / CopyPerViewConstantBufferData: the constant blocks PSMain reads
+void VQRenderer::FillSceneConstants(const FSceneView& SceneView, const FPostProcessParameters& PPParams,
+                                    const FEnvironmentMapRenderingResources& env, const FGraphicsSettings& GFXSettings,
+                                    bool bHDRDisplay, VqPerFrameData& PerFrame, VqPerViewLightingData& PerView) const {
     // CopyPerFrameConstantBufferData (SceneRendering.cpp:429-450)
-    VqPerFrameData PerFrame;
     std::memset(&PerFrame, 0, sizeof(PerFrame));
     PerFrame.Lights = SceneView.GPULightingData;
     PerFrame.fAmbientLightingFactor = SceneView.sceneRenderOptions.fAmbientLightingFactor;
@@ -193,16 +193,37 @@ bool VQRenderer::RenderSceneColor(cudaStream_t pCmd, const FSceneView& SceneView
     PerFrame.fHDRIOffsetInRadians = SceneView.HDRIYawOffset;
     if (bHDRDisplay) PerFrame.fAmbientLightingFactor *= 0.005f;
     // CopyPerViewConstantBufferData (SceneRendering.cpp:452-467)
-    VqPerViewLightingData PerView;
     std::memset(&PerView, 0, sizeof(PerView));
     PerView.CameraPosition = SceneView.cameraPosition;
     PerView.ScreenDimensions = {(float)PPParams.SceneRTWidth, (float)PPParams.SceneRTHeight};
     PerView.MaxEnvMapLODLevels = (float)env.GetNumSpecularIrradianceCubemapLODLevels();
     PerView.EnvironmentMapDiffuseOnlyIllumination = GFXSettings.Reflections == EReflections::SCREEN_SPACE_REFLECTIONS__FFX;
+}
+
+bool VQRenderer::RenderSceneColor(cudaStream_t pCmd, const FSceneView& SceneView, const FPostProcessParameters& PPParams,
+                                  const VqGBuffer& GBuffer, const FEnvironmentMapRenderingResources& env,
+                                  const FGraphicsSettings& GFXSettings, bool bHDRDisplay) {
+    VqPerFrameData PerFrame;
+    VqPerViewLightingData PerView;
+    FillSceneConstants(SceneView, PPParams, env, GFXSettings, bHDRDisplay, PerFrame, PerView);
     // IBL SRVs (SceneRendering.cpp:1690-1717): blurred diffuse irradiance, prefiltered specular, BRDF LUT
     VqEnvironmentMaps maps{env.DiffuseBlurred(), env.Specular(), mBRDFLUT.View()};
     VQ_TRY(vq_forward_lighting(mCtx, &PerFrame, &PerView, &GBuffer, &maps, mSceneColor.View(), 0, mSceneColor.height, pCmd),
            "vq_forward_lighting");
+    return true;
+}
+
+bool VQRenderer::RenderSceneColorFromMaterials(cudaStream_t pCmd, const FSceneView& SceneView, const FPostProcessParameters& PPParams,
+                                               const VqSurfaceInputs& SurfaceInputs, const VqMaterialTable* MaterialTable,
+                                               const FEnvironmentMapRenderingResources& env, const FGraphicsSettings& GFXSettings,
+                                               bool bHDRDisplay, bool bAlphaMask) {
+    VqPerFrameData PerFrame;
+    VqPerViewLightingData PerView;
+    FillSceneConstants(SceneView, PPParams, env, GFXSettings, bHDRDisplay, PerFrame, PerView);
+    VqEnvironmentMaps maps{env.DiffuseBlurred(), env.Specular(), mBRDFLUT.View()};
+    VQ_TRY(vq_forward_lighting_from_materials(mCtx, &PerFrame, &PerView, &SurfaceInputs, MaterialTable, bAlphaMask ? 1 : 0, &maps,
+                                              mSceneColor.View(), 0, mSceneColor.height, pCmd),
+           "vq_forward_lighting_from_materials");
     return true;
 }
 

@@ -232,6 +232,13 @@ public:
     bool RenderSceneColor(cudaStream_t pCmd, const FSceneView& SceneView, const FPostProcessParameters& PPParams,
                           const VqGBuffer& GBuffer, const FEnvironmentMapRenderingResources& env,
                           const FGraphicsSettings& GFXSettings, bool bHDR);
+    // RenderSceneColor with PSMain run end to end from what the rasteriser interpolates and the scene's materials (one launch,
+    // no G-buffer: vq_forward_lighting_from_materials); bAlphaMask selects the ENABLE_ALPHA_MASK variant. SceneColor must have
+    // the size of the attribute planes.
+    bool RenderSceneColorFromMaterials(cudaStream_t pCmd, const FSceneView& SceneView, const FPostProcessParameters& PPParams,
+                                       const VqSurfaceInputs& SurfaceInputs, const VqMaterialTable* MaterialTable,
+                                       const FEnvironmentMapRenderingResources& env, const FGraphicsSettings& GFXSettings,
+                                       bool bHDR, bool bAlphaMask = false);
     const VqImage* RenderPostProcess(cudaStream_t pCmd, const FPostProcessParameters& PPParams, bool bHDR);
     // "Draw Environment Map" (SceneRendering.cpp:1821-1850, Skydome.hlsl): fills the pixels of SceneColor that no surface
     // covered (normal plane == 0) with the equirect HDRI seen through EnvironmentMapViewProj (row-major, row-vector
@@ -248,6 +255,8 @@ public:
     const FTexture2D& BRDFIntegrationLUT() const { return mBRDFLUT; }
 
 private:
+    void FillSceneConstants(const FSceneView& SceneView, const FPostProcessParameters& PPParams, const FEnvironmentMapRenderingResources& env,
+                            const FGraphicsSettings& GFXSettings, bool bHDR, VqPerFrameData& PerFrame, VqPerViewLightingData& PerView) const;
     VqContext* mCtx = nullptr;
     FTexture2D mBRDFLUT;                                        // EProceduralTextures::IBL_BRDF_INTEGRATION_LUT
     FTexture2D mSceneColor, mBlurTemp, mBlurOut, mTonemapperOut, mCASOut, mEASUOut, mRCASOut;
