@@ -394,8 +394,8 @@ VQ_API int vq_gbuffer_from_materials(VqContext* ctx, const VqSurfaceInputs* in, 
  * fragment writes nothing. Rows [row_begin,row_end) follow vq_gbuffer_from_materials: quads are aligned to absolute even rows,
  * so row ranges tile the image. The defined deviations from the shader text are those of the two halves: the sampling rules
  * of vq_gbuffer_from_materials / VqSurfaceInputs and the K1 list at vq_forward_lighting. No shadow maps are bound (lit as
- * vq_forward_lighting lights them): the PCF pre-pass of vq_forward_lighting_shadowed needs the world position of every pixel
- * in device memory, which is the G-buffer this call does without. The arguments are checked before the device is touched.
+ * vq_forward_lighting lights them); vq_forward_lighting_shadowed_from_materials (SURVEY §8(f).4 below) is the same call with
+ * the shadow maps bound. The arguments are checked before the device is touched.
  * Like vq_forward_lighting, it rebuilds the IBL sampling copies per call unless the environment is registered. */
 VQ_API int vq_forward_lighting_from_materials(VqContext* ctx, const VqPerFrameData* per_frame,
                                               const VqPerViewLightingData* per_view, const VqSurfaceInputs* in,
@@ -499,6 +499,20 @@ VQ_API int vq_forward_lighting_shadowed(VqContext* ctx,
                                         VqImage out_color,
                                         int row_begin, int row_end,
                                         void* stream);
+/* vq_forward_lighting_from_materials with the shadow maps bound: computes what vq_gbuffer_from_materials (with an emissive
+ * plane) followed by vq_forward_lighting_shadowed(ctx, per_frame, per_view, &gb, env, shadow_maps, out_color, ...) computes,
+ * bit for bit (with the same yaw caveat as vq_forward_lighting_from_materials), in ONE launch: the PCF tests run inside the
+ * kernel on the positions and normals it has just produced, so neither the G-buffer nor the PCF records reach device memory
+ * and the call uses no context scratch beyond the environment's sampling copies (the one-stream rule of
+ * vq_forward_lighting_shadowed does not apply). Maps, caster lists and the f2*ShadowMapDimensions fields are read as
+ * vq_forward_lighting_shadowed reads them; when no test runs (no map bound for any caster type present) the result is
+ * vq_forward_lighting_from_materials's. Pixels the alpha mask discards are left untouched. Every argument is checked before
+ * the device is touched. */
+VQ_API int vq_forward_lighting_shadowed_from_materials(VqContext* ctx, const VqPerFrameData* per_frame,
+                                                       const VqPerViewLightingData* per_view, const VqSurfaceInputs* in,
+                                                       const VqMaterialTable* table, int alpha_mask, const VqEnvironmentMaps* env,
+                                                       const VqShadowMaps* shadow_maps, VqImage out_color,
+                                                       int row_begin, int row_end, void* stream);
 VQ_API int      vq_depth_pyramid_level_count(int width, int height);
 VQ_API uint64_t vq_depth_pyramid_texel_count(int width, int height, int levels);
 VQ_API int vq_depth_min_pyramid(VqContext* ctx, VqImage depth_r32f, void* levels, int n_levels, void* stream);

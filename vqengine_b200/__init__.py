@@ -34,7 +34,7 @@ ABI_SYMBOLS = [
     "vq_hdr_parse", "vq_hdr_decode", "vq_hdr_load_host", "vq_hdr_encode_rgbe", "vq_hdr_pack_file", "vq_hdr_save_host",
     "vq_skydome", "vq_apply_reflections", "vq_specular_prefilter_multi", "vq_specular_prefilter_ranges", "vq_forward_lighting_multi_signal", "vq_image_resize", "vq_resize_axis_table",
     "vq_forward_lighting_shadowed", "vq_depth_pyramid_level_count", "vq_depth_pyramid_texel_count", "vq_depth_min_pyramid",
-    "vq_forward_lighting_from_materials",
+    "vq_forward_lighting_from_materials", "vq_forward_lighting_shadowed_from_materials",
 ]
 
 
@@ -118,6 +118,8 @@ def _load() -> C.CDLL:
     lib.vq_apply_reflections.argtypes = [vp, Image, Image, P(Image), vp]
     lib.vq_forward_lighting_shadowed.argtypes = [vp, P(PerFrameData), P(PerViewLightingData), P(GBuffer), P(EnvironmentMaps),
                                                  P(ShadowMaps), Image, C.c_int, C.c_int, vp]
+    lib.vq_forward_lighting_shadowed_from_materials.argtypes = [vp, P(PerFrameData), P(PerViewLightingData), P(SurfaceInputs), vp,
+                                                                C.c_int, P(EnvironmentMaps), P(ShadowMaps), Image, C.c_int, C.c_int, vp]
     lib.vq_depth_pyramid_level_count.argtypes = [C.c_int, C.c_int]
     lib.vq_depth_pyramid_texel_count.argtypes = [C.c_int, C.c_int, C.c_int]
     lib.vq_depth_pyramid_texel_count.restype = C.c_uint64
@@ -267,6 +269,22 @@ def _stream_ptr(stream) -> C.c_void_p:
     return C.c_void_p(stream.cuda_stream)
 
 
+def _shadow_maps(point_cubes, spot_maps, directional_map) -> ShadowMaps:
+    """VqShadowMaps over point_cubes [casters,6,R,R], spot_maps [casters,H,W], directional_map [H,W] (contiguous float32 CUDA
+    tensors or None)"""
+    sm = ShadowMaps()
+    if point_cubes is not None:
+        assert point_cubes.is_contiguous() and point_cubes.dim() == 4 and point_cubes.shape[1] == 6 and point_cubes.shape[2] == point_cubes.shape[3]
+        sm.point_cubes, sm.point_res = point_cubes.data_ptr(), point_cubes.shape[2]
+    if spot_maps is not None:
+        assert spot_maps.is_contiguous() and spot_maps.dim() == 3
+        sm.spot_maps, sm.spot_width, sm.spot_height = spot_maps.data_ptr(), spot_maps.shape[2], spot_maps.shape[1]
+    if directional_map is not None:
+        assert directional_map.is_contiguous() and directional_map.dim() == 2
+        sm.directional_map, sm.directional_width, sm.directional_height = directional_map.data_ptr(), directional_map.shape[1], directional_map.shape[0]
+    return sm
+
+
 class Context:
     """Owns a VqContext (IRenderPass::Initialize / Destroy)."""
 
@@ -315,16 +333,7 @@ class Context:
     def forward_lighting_shadowed(self, per_frame, per_view, gbuffer: GBuffer, env: EnvironmentMaps, out, point_cubes=None,
                                   spot_maps=None, directional_map=None, row_begin=0, row_end=None, stream=None):
         """point_cubes [casters,6,R,R], spot_maps [casters,H,W], directional_map [H,W]: contiguous float32 CUDA tensors or None"""
-        sm = ShadowMaps()
-        if point_cubes is not None:
-            assert point_cubes.is_contiguous() and point_cubes.dim() == 4 and point_cubes.shape[1] == 6 and point_cubes.shape[2] == point_cubes.shape[3]
-            sm.point_cubes, sm.point_res = point_cubes.data_ptr(), point_cubes.shape[2]
-        if spot_maps is not None:
-            assert spot_maps.is_contiguous() and spot_maps.dim() == 3
-            sm.spot_maps, sm.spot_width, sm.spot_height = spot_maps.data_ptr(), spot_maps.shape[2], spot_maps.shape[1]
-        if directional_map is not None:
-            assert directional_map.is_contiguous() and directional_map.dim() == 2
-            sm.directional_map, sm.directional_width, sm.directional_height = directional_map.data_ptr(), directional_map.shape[1], directional_map.shape[0]
+        sm = _shadow_maps(point_cubes, spot_maps, directional_map)
         o = image_of(out)
         _check(lib.vq_forward_lighting_shadowed(self._h, C.byref(per_frame), C.byref(per_view), C.byref(gbuffer), C.byref(env),
                                                 C.byref(sm), o, row_begin, o.height if row_end is None else row_end, _stream_ptr(stream)))
@@ -369,6 +378,17 @@ class Context:
         _check(lib.vq_forward_lighting_from_materials(self._h, C.byref(per_frame), C.byref(per_view), C.byref(inputs), table._h,
                                                       1 if alpha_mask else 0, C.byref(env), image_of(out), row_begin,
                                                       h if row_end is None else row_end, _stream_ptr(stream)))
+
+    def forward_lighting_shadowed_from_materials(self, per_frame, per_view, inputs: SurfaceInputs, table: "MaterialTable",
+                                                 env: EnvironmentMaps, out, point_cubes=None, spot_maps=None, directional_map=None,
+                                                 alpha_mask: bool = False, row_begin=0, row_end=None, stream=None):
+        """forward_lighting_from_materials with the shadow maps bound (maps as forward_lighting_shadowed takes them): one launch,
+        no G-buffer, no PCF records"""
+        sm = _shadow_maps(point_cubes, spot_maps, directional_map)
+        h = inputs.position_u.height
+        _check(lib.vq_forward_lighting_shadowed_from_materials(self._h, C.byref(per_frame), C.byref(per_view), C.byref(inputs), table._h,
+                                                               1 if alpha_mask else 0, C.byref(env), C.byref(sm), image_of(out),
+                                                               row_begin, h if row_end is None else row_end, _stream_ptr(stream)))
 
     # SURVEY 8(f).2: Radiance .hdr
     def hdr_decode(self, file_bytes: bytes, stream=None):

@@ -17,6 +17,7 @@
 //   * cubemap taps are seamless across face edges, so face selection is not a discontinuity.
 #include "vq_common.cuh"
 #include "vq_surface_sample.cuh"
+#include "vq_shadow_math.cuh"
 #include <stdlib.h>
 
 using namespace vq;
@@ -179,7 +180,7 @@ struct Px2 {
     f2 a2gV, gV;                  // a2 * G1(V), G1(V) = Smith-Schlick-GGX of the view vector (BRDF.hlsl:82-97)
     f2 k4, omk;                   // k + 0.0001, 1 - k with k = (roughness+1)^2 / 8
     uint32_t texA, texB;          // shared-memory addresses of the two pixels' position texels (planes follow at FWD_PLANE)
-    uint64_t recA, recB;          // SHADOWED only: the two pixels' PCF records (ShadowRecV, vq_common.cuh)
+    uint64_t recA, recB;          // SHADOWED forward_kernel only: the two pixels' PCF records (ShadowRecV, vq_common.cuh)
 };
 struct Acc2 { f2 ax, ay, az, bx, by, bz, cx, cy, cz; };   // sum over lights of w*col * {(1-fc), fc*spec, spec}
 
@@ -332,15 +333,25 @@ __device__ __forceinline__ LightVec2 light_vector2(const Px2& s, float3 pos) {
     return L;
 }
 
+// REC_SMEM (psmain_kernel): the pixels' PCF records are not in Px2 but in shared memory, PS_REC_PLANE bytes past each pixel's
+// position texel (a fifth plane of the stage, 8 of its 16 bytes used), and are read where a caster needs them: two LDS.64 per
+// caster light instead of four registers live across the whole light loop, which the fused kernel's budget has no room for.
+constexpr uint32_t PS_REC_PLANE = 4u * FWD_PLANE;
+__device__ __forceinline__ uint64_t lds64(uint32_t addr) {       // volatile: read at the point of use, not hoisted out of the loop
+    uint64_t r; asm volatile("ld.shared.u64 %0, [%1];" : "=l"(r) : "r"(addr) : "memory"); return r;
+}
+
 // SHADOWED: the shadow factor pair {pixel A, pixel B} of caster slot c = 1 - taps/n (Lighting.hlsl:162-164, :207-209), taps from the
 // pixels' PCF records; a continuous factor of the light's weight, so one FMA instead of the reference's division
+template <bool REC_SMEM>
 __device__ __forceinline__ f2 shadow_factor2(const Px2& s, int slot, float invTaps) {
-    const float ca = (float)((uint32_t)(s.recA >> (5 * slot)) & 31u), cb = (float)((uint32_t)(s.recB >> (5 * slot)) & 31u);
+    const uint64_t ra = REC_SMEM ? lds64(s.texA + PS_REC_PLANE) : s.recA, rb = REC_SMEM ? lds64(s.texB + PS_REC_PLANE) : s.recB;
+    const float ca = (float)((uint32_t)(ra >> (5 * slot)) & 31u), cb = (float)((uint32_t)(rb >> (5 * slot)) & 31u);
     return fma2(mk(ca, cb), bc(-invTaps), bc(1.0f));
 }
 
 // every light of the frame for one pixel pair, in PSMain's order
-template <bool TINY, bool SHADOWED>
+template <bool TINY, bool SHADOWED, bool REC_SMEM>
 __device__ __forceinline__ void shade_all_lights(const Px2& s, Acc2& acc, const FwdParams& P) {
     const float3 cam = P.cam;
     const int numPoint = P.numPoint, numSpot = P.numSpot;
@@ -354,7 +365,7 @@ __device__ __forceinline__ void shade_all_lights(const Px2& s, Acc2& acc, const 
         f2 scale = mk(L.d2.v.x < l.d2Limit ? att.v.x : 0.0f, L.d2.v.y < l.d2Limit ? att.v.y : 0.0f);
         if (SHADOWED) {                                                   // OmnidirectionalShadowTestPCF: 20 taps
             const int c = i - (numPoint - P.shadow.nPointCasters);
-            if (c >= 0) scale = scale * shadow_factor2(s, c, 1.0f / 20.0f);
+            if (c >= 0) scale = scale * shadow_factor2<REC_SMEM>(s, c, 1.0f / 20.0f);
         }
         shade_light2<TINY>(s, acc, cam, L.x, L.y, L.z, L.d2, L.invD, scale, l.color);
     }
@@ -379,7 +390,7 @@ __device__ __forceinline__ void shade_all_lights(const Px2& s, Acc2& acc, const 
         f2 scale = mk(inten[0], inten[1]) * bc(l.brightness) * (L.invD * L.invD);
         if (SHADOWED) {                                                   // ShadowTestPCF: 5x5 taps
             const int c = k - (numSpot - P.shadow.nSpotCasters);
-            if (c >= 0) scale = scale * shadow_factor2(s, P.shadow.nPointCasters + c, 1.0f / 25.0f);
+            if (c >= 0) scale = scale * shadow_factor2<REC_SMEM>(s, P.shadow.nPointCasters + c, 1.0f / 25.0f);
         }
         shade_light2<TINY>(s, acc, cam, L.x, L.y, L.z, L.d2, L.invD, scale, l.color);
     }
@@ -387,7 +398,7 @@ __device__ __forceinline__ void shade_all_lights(const Px2& s, Acc2& acc, const 
     if (P.dirEnabled) {
         const SDir d = P.dir;
         f2 scale = bc(1.0f);
-        if (SHADOWED) { if (P.shadow.dirSlot >= 0) scale = shadow_factor2(s, P.shadow.dirSlot, 1.0f / 25.0f); }
+        if (SHADOWED) { if (P.shadow.dirSlot >= 0) scale = shadow_factor2<REC_SMEM>(s, P.shadow.dirSlot, 1.0f / 25.0f); }
         shade_light2<TINY>(s, acc, cam, bc(d.wi.x), bc(d.wi.y), bc(d.wi.z), bc(1.0f), bc(1.0f), scale, d.radiance);
     }
 }
@@ -651,7 +662,7 @@ __device__ __forceinline__ void finish_pair(const FwdParams& P, const FaceRec* _
 }
 
 // per-pixel-pair set-up (everything the lights share) and the light loops: fills s, acc, roughness, ao from the staged texels
-template <bool SHADOWED>
+template <bool SHADOWED, bool REC_SMEM = false>
 __device__ __forceinline__ void shade_pair_lights(const FwdParams& P, Px2& s, Acc2& acc, f2& roughness, f2& ao) {
     {
         const float4 pa = lds128(s.texA), pb = lds128(s.texB);
@@ -688,9 +699,9 @@ __device__ __forceinline__ void shade_pair_lights(const FwdParams& P, Px2& s, Ac
     const f2 tmin = bc(1.0f) + mk(fminf(s.a2m1.v.x, 0.0f), fminf(s.a2m1.v.y, 0.0f));
     const f2 dmin = bc(PI) * (tmin * tmin);
     if (__any_sync(0xffffffffu, fminf(dmin.v.x, dmin.v.y) < 2e-12f))
-        shade_all_lights<true, SHADOWED>(s, acc, P);
+        shade_all_lights<true, SHADOWED, REC_SMEM>(s, acc, P);
     else
-        shade_all_lights<false, SHADOWED>(s, acc, P);
+        shade_all_lights<false, SHADOWED, REC_SMEM>(s, acc, P);
 }
 
 // entry i = face*16 + mip of the specular cube's face table, staged once per CTA: the lanes of a warp mostly share the face and
@@ -797,11 +808,23 @@ __global__ void __launch_bounds__(FWD_THREADS, FWD_CTAS_PER_SM) forward_kernel(c
 // PSMain end to end: the surface producer and K1 fused, with the G-buffer in shared memory instead of HBM
 // ---------------------------------------------------------------------------------------------
 struct PsParams {
-    FwdParams F;                       // K1's frame (outs[0] = the destination; no G-buffer planes, no shadow records)
+    FwdParams F;                       // K1's frame (outs[0] = the destination; no G-buffer planes; SHADOWED: F.shadow holds the
+                                       // caster counts and dirSlot, its record pointer stays null)
     SurfArgs S;                        // the surface producer's inputs (no G-buffer outputs)
+    vqshadow::ShadowLights L;          // SHADOWED only: what the PCF tests read besides the pixel (last, so that the unshadowed
+                                       // instantiations read F and S at the same offsets)
 };
 __device__ __forceinline__ void sts128(uint32_t addr, float4 v) {
     asm volatile("st.shared.v4.f32 [%0], {%1,%2,%3,%4};" :: "r"(addr), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w) : "memory");
+}
+// The PCF record of a staged pixel: exactly what shadow_pcf_kernel computes from the G-buffer texels the stage holds (position =
+// plane 0 .xyz, the normal-mapped normal = plane 1 .xyz). Every lane of the warp must call it (pcf_record votes across the warp).
+__device__ __forceinline__ uint64_t staged_pcf_record(const vqshadow::ShadowLights& L, uint32_t texel) {
+    const float4 p = lds128(texel), n = lds128(texel + FWD_PLANE);
+    vqshadow::Px4 p4, n4;
+    p4.x = p.x; p4.y = p.y; p4.z = p.z; p4.w = p.w;
+    n4.x = n.x; n4.y = n.y; n4.z = n.z; n4.w = n.w;
+    return vqshadow::pcf_record(L, p4, n4);
 }
 
 // A persistent CTA walks tiles of 2 rows x FWD_THREADS columns (rows aligned to absolute even rows, as the surface producer's
@@ -812,12 +835,14 @@ __device__ __forceinline__ void sts128(uint32_t addr, float4 v) {
 //             pixel was produced (inside the image and the row range, not discarded by the alpha mask);
 //   shading:  thread t shades the pixel pair (row 0, column t), (row 1, column t) with K1's code on the stage and stores the
 //             pixels that were produced. The lane-pair gathers pair neighbouring columns of one row, as in K1.
+//             SHADOWED: first the PCF records of both pixels from the stage (all 128 threads: a warp is 32 consecutive columns of
+//             one row, as in shadow_pcf_kernel), then the shadowed light loop on them.
 // The phases stay sequential: a warp-specialised K1 measured slower (DESIGN.md §4).
-template <bool ROT>
+template <bool ROT, bool SHADOWED>
 __global__ void __launch_bounds__(FWD_THREADS, FWD_CTAS_PER_SM) psmain_kernel(const __grid_constant__ PsParams Q) {
     const FwdParams& P = Q.F;
     const SurfArgs& A = Q.S;
-    __shared__ __align__(128) float4 sStage[4 * FWD_TILE];
+    __shared__ __align__(128) float4 sStage[(SHADOWED ? 5 : 4) * FWD_TILE];       // SHADOWED: + the PCF records (PS_REC_PLANE)
     __shared__ FaceRec sFace[16 * 8];
     __shared__ uint8_t sProduced[FWD_TILE];
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -854,7 +879,17 @@ __global__ void __launch_bounds__(FWD_THREADS, FWD_CTAS_PER_SM) psmain_kernel(co
         s.texB = s.texA + FWD_THREADS * 16u;
         f2 roughness, ao;
         Acc2 acc;
-        shade_pair_lights<false>(P, s, acc, roughness, ao);
+        if (SHADOWED) {                                           // one copy of the PCF code, run for pixel A then pixel B
+            // lanes off a ragged row alias its last pixel and store the same record there (the axis path gives the general
+            // count, so the warp a lane sits in does not change it); a record is only read by the threads that stored it
+#pragma unroll 1
+            for (int k = 0; k < 2; ++k) {
+                const uint32_t texel = k ? s.texB : s.texA;
+                const uint64_t rec = staged_pcf_record(Q.L, texel);
+                asm volatile("st.shared.u64 [%0], %1;" :: "r"(texel + PS_REC_PLANE), "l"(rec) : "memory");
+            }
+        }
+        shade_pair_lights<SHADOWED, SHADOWED>(P, s, acc, roughness, ao);
         const bool validA = inRow && sProduced[tid] != 0, validB = inRow && sProduced[FWD_THREADS + tid] != 0;
         if (P.diffuseOnly) finish_pair<false, ROT, false>(P, sFace, s, acc, roughness, ao, y0, xA, y0 + 1, xA, validA, validB);
         else finish_pair<false, ROT, true>(P, sFace, s, acc, roughness, ao, y0, xA, y0 + 1, xA, validA, validB);
@@ -1141,17 +1176,25 @@ extern "C" int vq_forward_lighting_multi_signal(VqContext* ctx, const VqPerFrame
 }
 
 // PSMain from interpolants and materials in one launch (psmain_kernel): what vq_gbuffer_from_materials with an emissive plane
-// followed by vq_forward_lighting computes, without the G-buffer. The arguments are checked before the device is touched.
-extern "C" int vq_forward_lighting_from_materials(VqContext* ctx, const VqPerFrameData* pf, const VqPerViewLightingData* pv,
-                                                  const VqSurfaceInputs* in, const VqMaterialTable* table, int alpha_mask,
-                                                  const VqEnvironmentMaps* env, VqImage out, int row_begin, int row_end, void* stream) {
+// followed by vq_forward_lighting (sm == nullptr) or vq_forward_lighting_shadowed computes, without the G-buffer. The arguments are
+// checked before the device is touched.
+static int psmain_launch(VqContext* ctx, const VqPerFrameData* pf, const VqPerViewLightingData* pv, const VqSurfaceInputs* in,
+                         const VqMaterialTable* table, int alpha_mask, const VqEnvironmentMaps* env, const VqShadowMaps* sm,
+                         VqImage out, int row_begin, int row_end, void* stream) {
     VQ_REQUIRE(pf && pv && env && in, "null argument");
     const int W = in->position_u.width, H = in->position_u.height;
     VQ_REQUIRE(vq_image_ok(out) && out.width == W && out.height == H, "the output must have the size of the attribute planes");
     static_assert(sizeof(PsParams) <= 32764, "kernel parameter space");
     PsParams Q;
     memset(&Q, 0, sizeof(Q));
-    int rc = surface_inputs(in, table, pf->fAmbientLightingFactor, alpha_mask, row_begin, row_end, Q.S); if (rc) return rc;
+    int rc;
+    bool shadowed = false;                                        // does any PCF test run?
+    if (sm) {
+        rc = vq_shadow_maps_check(pf->Lights, *sm); if (rc) return rc;
+        shadowed = vq_shadow_slots(pf->Lights, *sm, Q.F.shadow);  // no test runs: every factor is 1, the unshadowed kernel
+        if (shadowed) vqshadow::fill_shadow_lights(Q.L, *pf, *pv, *sm);
+    }
+    rc = surface_inputs(in, table, pf->fAmbientLightingFactor, alpha_mask, row_begin, row_end, Q.S); if (rc) return rc;
     VQ_REQUIRE(light_counts_ok(pf->Lights), "light counts exceed the cbuffer arrays");
     rc = vq_enter(ctx); if (rc) return rc;
     VQ_MARK("RenderSceneColor");
@@ -1169,9 +1212,32 @@ extern "C" int vq_forward_lighting_from_materials(VqContext* ctx, const VqPerFra
     if (gy < 1) gy = 1;
     if (gy > pairs) gy = pairs;
     const bool rot = P.sinB != 0.0f || P.cosB != 1.0f;
-    if (rot) psmain_kernel<true><<<dim3(gx, gy), FWD_THREADS, 0, (cudaStream_t)stream>>>(Q);
-    else psmain_kernel<false><<<dim3(gx, gy), FWD_THREADS, 0, (cudaStream_t)stream>>>(Q);
-    return vq_check_launch("forward_lighting_from_materials");
+    const dim3 grid(gx, gy);
+    const cudaStream_t s = (cudaStream_t)stream;
+    if (shadowed) {
+        if (rot) psmain_kernel<true, true><<<grid, FWD_THREADS, 0, s>>>(Q);
+        else psmain_kernel<false, true><<<grid, FWD_THREADS, 0, s>>>(Q);
+    } else {
+        if (rot) psmain_kernel<true, false><<<grid, FWD_THREADS, 0, s>>>(Q);
+        else psmain_kernel<false, false><<<grid, FWD_THREADS, 0, s>>>(Q);
+    }
+    return vq_check_launch(sm ? "forward_lighting_shadowed_from_materials" : "forward_lighting_from_materials");
+}
+
+extern "C" int vq_forward_lighting_from_materials(VqContext* ctx, const VqPerFrameData* pf, const VqPerViewLightingData* pv,
+                                                  const VqSurfaceInputs* in, const VqMaterialTable* table, int alpha_mask,
+                                                  const VqEnvironmentMaps* env, VqImage out, int row_begin, int row_end, void* stream) {
+    return psmain_launch(ctx, pf, pv, in, table, alpha_mask, env, nullptr, out, row_begin, row_end, stream);
+}
+
+// The same with the shadow maps bound: the PCF tests run inside psmain_kernel on the staged positions and normals, so there are no
+// PCF records in device memory and no context scratch beyond what the unshadowed call uses.
+extern "C" int vq_forward_lighting_shadowed_from_materials(VqContext* ctx, const VqPerFrameData* pf, const VqPerViewLightingData* pv,
+                                                           const VqSurfaceInputs* in, const VqMaterialTable* table, int alpha_mask,
+                                                           const VqEnvironmentMaps* env, const VqShadowMaps* sm, VqImage out,
+                                                           int row_begin, int row_end, void* stream) {
+    VQ_REQUIRE(sm, "null shadow maps");
+    return psmain_launch(ctx, pf, pv, in, table, alpha_mask, env, sm, out, row_begin, row_end, stream);
 }
 
 // The IBL cubemaps and the BRDF LUT are sampled from footprint-friendly copies (see CubeV, LutV).

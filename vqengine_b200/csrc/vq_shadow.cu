@@ -131,6 +131,23 @@ __global__ void __launch_bounds__(256) depth_min6_kernel(const __grid_constant__
 
 }  // namespace
 
+int vq_shadow_maps_check(const VqSceneLighting& L, const VqShadowMaps& sm) {
+    VQ_REQUIRE(L.numPointCasters >= 0 && L.numPointCasters <= VQ_NUM_SHADOWING_LIGHTS_POINT &&
+               L.numSpotCasters >= 0 && L.numSpotCasters <= VQ_NUM_SHADOWING_LIGHTS_SPOT, "caster counts exceed the cbuffer arrays");
+    // texel indices inside one map are 32-bit in the kernel
+    if (sm.point_cubes) VQ_REQUIRE(sm.point_res > 0 && sm.point_res <= 16384, "point shadow cubes need a resolution in 1..16384");
+    if (sm.spot_maps) VQ_REQUIRE(sm.spot_width > 0 && sm.spot_height > 0 && (uint64_t)sm.spot_width * sm.spot_height < (1ull << 31), "spot shadow maps need positive dimensions (< 2^31 texels)");
+    if (sm.directional_map) VQ_REQUIRE(sm.directional_width > 0 && sm.directional_height > 0 && (uint64_t)sm.directional_width * sm.directional_height < (1ull << 31), "directional shadow map needs positive dimensions (< 2^31 texels)");
+    return VQ_OK;
+}
+
+bool vq_shadow_slots(const VqSceneLighting& L, const VqShadowMaps& sm, vq::ShadowRecV& v) {
+    const bool dirTest = sm.directional_map && L.directional.enabled && L.directional.shadowing;
+    v.nPointCasters = L.numPointCasters; v.nSpotCasters = L.numSpotCasters;
+    v.dirSlot = dirTest ? L.numPointCasters + L.numSpotCasters : -1;
+    return (sm.point_cubes && L.numPointCasters > 0) || (sm.spot_maps && L.numSpotCasters > 0) || dirTest;
+}
+
 extern "C" int vq_forward_lighting_shadowed(VqContext* ctx, const VqPerFrameData* pf, const VqPerViewLightingData* pv,
                                             const VqGBuffer* gb, const VqEnvironmentMaps* env, const VqShadowMaps* sm,
                                             VqImage out, int row_begin, int row_end, void* stream) {
@@ -138,14 +155,9 @@ extern "C" int vq_forward_lighting_shadowed(VqContext* ctx, const VqPerFrameData
     VQ_MARK("RenderSceneColor");
     VQ_REQUIRE(pf && pv && gb && env && sm, "null parameter block");
     const VqSceneLighting& L = pf->Lights;
-    VQ_REQUIRE(L.numPointCasters >= 0 && L.numPointCasters <= VQ_NUM_SHADOWING_LIGHTS_POINT &&
-               L.numSpotCasters >= 0 && L.numSpotCasters <= VQ_NUM_SHADOWING_LIGHTS_SPOT, "caster counts exceed the cbuffer arrays");
-    // texel indices inside one map are 32-bit in the kernel
-    if (sm->point_cubes) VQ_REQUIRE(sm->point_res > 0 && sm->point_res <= 16384, "point shadow cubes need a resolution in 1..16384");
-    if (sm->spot_maps) VQ_REQUIRE(sm->spot_width > 0 && sm->spot_height > 0 && (uint64_t)sm->spot_width * sm->spot_height < (1ull << 31), "spot shadow maps need positive dimensions (< 2^31 texels)");
-    if (sm->directional_map) VQ_REQUIRE(sm->directional_width > 0 && sm->directional_height > 0 && (uint64_t)sm->directional_width * sm->directional_height < (1ull << 31), "directional shadow map needs positive dimensions (< 2^31 texels)");
-    const bool anyTest = (sm->point_cubes && L.numPointCasters > 0) || (sm->spot_maps && L.numSpotCasters > 0) ||
-                         (sm->directional_map && L.directional.enabled && L.directional.shadowing);
+    rc = vq_shadow_maps_check(L, *sm); if (rc) return rc;
+    vq::ShadowRecV V;
+    const bool anyTest = vq_shadow_slots(L, *sm, V);
     if (!anyTest || row_begin >= row_end)          // no test runs: every factor is 1, which is what the plain kernel computes
         return vq_forward_launch(ctx, pf, pv, gb, env, out, row_begin, row_end, (cudaStream_t)stream);
     VQ_REQUIRE(gb->position_ao.ptr && vq_image_ok(gb->position_ao) && vq_image_ok(gb->normal_roughness) &&
@@ -170,10 +182,7 @@ extern "C" int vq_forward_lighting_shadowed(VqContext* ctx, const VqPerFrameData
     shadow_pcf_kernel<<<dim3(gx, gy), 128, 0, (cudaStream_t)stream>>>(P);
     rc = vq_check_launch("shadow_pcf"); if (rc) return rc;
 
-    vq::ShadowRecV V;
     V.p = P.rec; V.pitch = P.recPitch;
-    V.nPointCasters = L.numPointCasters; V.nSpotCasters = L.numSpotCasters;
-    V.dirSlot = (sm->directional_map && L.directional.enabled && L.directional.shadowing) ? L.numPointCasters + L.numSpotCasters : -1;
     return vq_forward_launch(ctx, pf, pv, gb, env, out, row_begin, row_end, (cudaStream_t)stream, &V);
 }
 

@@ -228,6 +228,43 @@ bool VQRenderer::RenderSceneColorFromMaterials(cudaStream_t pCmd, const FSceneVi
 }
 
 // 4x4 inverse in double (row-major; the convention does not matter for an inverse), rounded to fp32 at the end
+// the shadow-map sizes the shader divides by (Lighting.hlsl:190, :237) are those of the maps bound; a light type without a map
+// keeps the engine's constant
+static void SetShadowMapDimensions(const VqShadowMaps& maps, VqPerFrameData& PerFrame) {
+    if (maps.point_cubes) PerFrame.f2PointLightShadowMapDimensions = {(float)maps.point_res, (float)maps.point_res};
+    if (maps.spot_maps) PerFrame.f2SpotLightShadowMapDimensions = {(float)maps.spot_width, (float)maps.spot_height};
+    if (maps.directional_map) PerFrame.f2DirectionalLightShadowMapDimensions = {(float)maps.directional_width, (float)maps.directional_height};
+}
+
+bool VQRenderer::RenderSceneColor(cudaStream_t pCmd, const FSceneView& SceneView, const FPostProcessParameters& PPParams,
+                                  const VqGBuffer& GBuffer, const FEnvironmentMapRenderingResources& env,
+                                  const FGraphicsSettings& GFXSettings, bool bHDRDisplay, const VqShadowMaps& ShadowMaps) {
+    VqPerFrameData PerFrame;
+    VqPerViewLightingData PerView;
+    FillSceneConstants(SceneView, PPParams, env, GFXSettings, bHDRDisplay, PerFrame, PerView);
+    SetShadowMapDimensions(ShadowMaps, PerFrame);
+    VqEnvironmentMaps maps{env.DiffuseBlurred(), env.Specular(), mBRDFLUT.View()};
+    VQ_TRY(vq_forward_lighting_shadowed(mCtx, &PerFrame, &PerView, &GBuffer, &maps, &ShadowMaps, mSceneColor.View(), 0,
+                                        mSceneColor.height, pCmd),
+           "vq_forward_lighting_shadowed");
+    return true;
+}
+
+bool VQRenderer::RenderSceneColorFromMaterials(cudaStream_t pCmd, const FSceneView& SceneView, const FPostProcessParameters& PPParams,
+                                               const VqSurfaceInputs& SurfaceInputs, const VqMaterialTable* MaterialTable,
+                                               const FEnvironmentMapRenderingResources& env, const FGraphicsSettings& GFXSettings,
+                                               bool bHDRDisplay, const VqShadowMaps& ShadowMaps, bool bAlphaMask) {
+    VqPerFrameData PerFrame;
+    VqPerViewLightingData PerView;
+    FillSceneConstants(SceneView, PPParams, env, GFXSettings, bHDRDisplay, PerFrame, PerView);
+    SetShadowMapDimensions(ShadowMaps, PerFrame);
+    VqEnvironmentMaps maps{env.DiffuseBlurred(), env.Specular(), mBRDFLUT.View()};
+    VQ_TRY(vq_forward_lighting_shadowed_from_materials(mCtx, &PerFrame, &PerView, &SurfaceInputs, MaterialTable, bAlphaMask ? 1 : 0,
+                                                       &maps, &ShadowMaps, mSceneColor.View(), 0, mSceneColor.height, pCmd),
+           "vq_forward_lighting_shadowed_from_materials");
+    return true;
+}
+
 static bool Invert4x4(const float m[16], float out[16]) {
     double a[4][8];
     for (int r = 0; r < 4; ++r)

@@ -239,6 +239,15 @@ public:
                                        const VqSurfaceInputs& SurfaceInputs, const VqMaterialTable* MaterialTable,
                                        const FEnvironmentMapRenderingResources& env, const FGraphicsSettings& GFXSettings,
                                        bool bHDR, bool bAlphaMask = false);
+    // The same two passes with the engine's shadow maps bound (ForwardLighting.hlsl:87-89, 321-377): vq_forward_lighting_shadowed
+    // and vq_forward_lighting_shadowed_from_materials. The f2*ShadowMapDimensions constants are those of the bound maps.
+    bool RenderSceneColor(cudaStream_t pCmd, const FSceneView& SceneView, const FPostProcessParameters& PPParams,
+                          const VqGBuffer& GBuffer, const FEnvironmentMapRenderingResources& env,
+                          const FGraphicsSettings& GFXSettings, bool bHDR, const VqShadowMaps& ShadowMaps);
+    bool RenderSceneColorFromMaterials(cudaStream_t pCmd, const FSceneView& SceneView, const FPostProcessParameters& PPParams,
+                                       const VqSurfaceInputs& SurfaceInputs, const VqMaterialTable* MaterialTable,
+                                       const FEnvironmentMapRenderingResources& env, const FGraphicsSettings& GFXSettings,
+                                       bool bHDR, const VqShadowMaps& ShadowMaps, bool bAlphaMask = false);
     const VqImage* RenderPostProcess(cudaStream_t pCmd, const FPostProcessParameters& PPParams, bool bHDR);
     // "Draw Environment Map" (SceneRendering.cpp:1821-1850, Skydome.hlsl): fills the pixels of SceneColor that no surface
     // covered (normal plane == 0) with the equirect HDRI seen through EnvironmentMapViewProj (row-major, row-vector
