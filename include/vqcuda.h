@@ -18,7 +18,7 @@
  *       vq_forward_lighting* with an environment that is NOT registered by
  *       vq_environment_prepare (the sampling copies are rebuilt into per-context scratch),
  *       vq_environment_prepare itself, vq_image_resize, vq_depth_min_pyramid,
- *       vq_forward_lighting_shadowed (per-pixel PCF records),
+ *       vq_forward_lighting_shadowed and vq_forward_lighting_shadowed_multi_signal (per-pixel PCF records),
  *       vq_forward_lighting_host.
  *     Synchronisation is the caller's (cudaStreamSynchronize == fence wait), except the
  *     *_host convenience calls which block.
@@ -170,6 +170,35 @@ VQ_API int vq_forward_lighting_multi(VqContext* ctx,
 VQ_API int vq_forward_lighting_multi_signal(VqContext* ctx, const VqPerFrameData* per_frame, const VqPerViewLightingData* per_view,
                                             const VqGBuffer* gbuffer, const VqEnvironmentMaps* env, const VqImage* outs, int n_outs,
                                             int dst_row_offset, int row_begin, int row_end, const VqPeerSignal* signal, void* stream);
+/* The other shading calls in the same multi-destination form. Into each of the n_outs (1..8) destinations, each call computes
+ * what its single-destination call computes into its one output, bit for bit, at rows offset by dst_row_offset; rows outside
+ * [row_begin,row_end) are not touched. With several destinations the pass runs as one kernel whose last CTA runs the rendezvous
+ * when `signal` is given (NULL: no rendezvous). Refused with VQ_ERR_INVALID_ARG before
+ * the device is touched, with vq_forward_lighting_multi_signal's messages: n_outs outside 1..8, a destination narrower or wider
+ * than the source or without dst_row_offset + height rows, a negative offset, a signal with n_ranks > 1 and one destination or an
+ * empty row range, and the shadow-map checks of vq_forward_lighting_shadowed.
+ *   vq_forward_lighting_shadowed_multi_signal: vq_forward_lighting_shadowed (the PCF pre-pass, then the shadowed forward kernel
+ *     with the multi-destination stores: two launches). The PCF records are context scratch, so calls on ONE context must be
+ *     issued on one stream at a time, as for vq_forward_lighting_shadowed. The environment is checked after the PCF launch.
+ *   vq_forward_lighting_from_materials_multi_signal: vq_forward_lighting_from_materials (shadow_maps NULL) or
+ *     vq_forward_lighting_shadowed_from_materials, one launch and no context scratch; when no PCF test would run it is the
+ *     unshadowed call. Pixels the alpha mask discards stay untouched in every destination. dst_row_offset must be even:
+ *     the surface producer's quads sit on even rows of the attribute planes, and the texture LOD of a rank's band matches the
+ *     whole frame's only if those rows are even rows of the frame too. A rank may pass the whole frame's attribute planes with its
+ *     row range and offset 0, or planes holding just its band with rows [0, band) and offset = the band's first row (even); in
+ *     the second form the SSAO plane wraps at the band's last row, not the frame's. */
+struct VqShadowMaps; struct VqSurfaceInputs; struct VqMaterialTable;     /* defined below (SURVEY §8(f).1 and §8(f).4) */
+VQ_API int vq_forward_lighting_shadowed_multi_signal(VqContext* ctx, const VqPerFrameData* per_frame,
+                                                     const VqPerViewLightingData* per_view, const VqGBuffer* gbuffer,
+                                                     const VqEnvironmentMaps* env, const struct VqShadowMaps* shadow_maps,
+                                                     const VqImage* outs, int n_outs, int dst_row_offset, int row_begin, int row_end,
+                                                     const VqPeerSignal* signal, void* stream);
+VQ_API int vq_forward_lighting_from_materials_multi_signal(VqContext* ctx, const VqPerFrameData* per_frame,
+                                                           const VqPerViewLightingData* per_view, const struct VqSurfaceInputs* in,
+                                                           const struct VqMaterialTable* table, int alpha_mask,
+                                                           const VqEnvironmentMaps* env, const struct VqShadowMaps* shadow_maps,
+                                                           const VqImage* outs, int n_outs, int dst_row_offset, int row_begin,
+                                                           int row_end, const VqPeerSignal* signal, void* stream);
 
 /* The forward pass samples the IBL cubemaps from bordered copies (each face carries a 1-texel border of its
  * neighbours, so seamless bilinear taps never leave the face). vq_environment_prepare builds those copies once and

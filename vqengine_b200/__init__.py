@@ -35,6 +35,7 @@ ABI_SYMBOLS = [
     "vq_skydome", "vq_apply_reflections", "vq_specular_prefilter_multi", "vq_specular_prefilter_ranges", "vq_forward_lighting_multi_signal", "vq_image_resize", "vq_resize_axis_table",
     "vq_forward_lighting_shadowed", "vq_depth_pyramid_level_count", "vq_depth_pyramid_texel_count", "vq_depth_min_pyramid",
     "vq_forward_lighting_from_materials", "vq_forward_lighting_shadowed_from_materials",
+    "vq_forward_lighting_shadowed_multi_signal", "vq_forward_lighting_from_materials_multi_signal",
 ]
 
 
@@ -120,6 +121,11 @@ def _load() -> C.CDLL:
                                                  P(ShadowMaps), Image, C.c_int, C.c_int, vp]
     lib.vq_forward_lighting_shadowed_from_materials.argtypes = [vp, P(PerFrameData), P(PerViewLightingData), P(SurfaceInputs), vp,
                                                                 C.c_int, P(EnvironmentMaps), P(ShadowMaps), Image, C.c_int, C.c_int, vp]
+    lib.vq_forward_lighting_shadowed_multi_signal.argtypes = [vp, P(PerFrameData), P(PerViewLightingData), P(GBuffer), P(EnvironmentMaps),
+                                                              P(ShadowMaps), P(Image), C.c_int, C.c_int, C.c_int, C.c_int, P(PeerSignal), vp]
+    lib.vq_forward_lighting_from_materials_multi_signal.argtypes = [vp, P(PerFrameData), P(PerViewLightingData), P(SurfaceInputs), vp,
+                                                                    C.c_int, P(EnvironmentMaps), P(ShadowMaps), P(Image), C.c_int,
+                                                                    C.c_int, C.c_int, C.c_int, P(PeerSignal), vp]
     lib.vq_depth_pyramid_level_count.argtypes = [C.c_int, C.c_int]
     lib.vq_depth_pyramid_texel_count.argtypes = [C.c_int, C.c_int, C.c_int]
     lib.vq_depth_pyramid_texel_count.restype = C.c_uint64
@@ -338,6 +344,19 @@ class Context:
         _check(lib.vq_forward_lighting_shadowed(self._h, C.byref(per_frame), C.byref(per_view), C.byref(gbuffer), C.byref(env),
                                                 C.byref(sm), o, row_begin, o.height if row_end is None else row_end, _stream_ptr(stream)))
 
+    def forward_lighting_shadowed_multi(self, per_frame, per_view, gbuffer: GBuffer, env: EnvironmentMaps, out_images, dst_row_offset,
+                                        point_cubes=None, spot_maps=None, directional_map=None, row_begin=0, row_end=None,
+                                        stream=None, signal: "PeerSignal" = None):
+        """forward_lighting_shadowed into several frames, as forward_lighting_multi stores them (out_images: local frame first, then
+        the peers' mapped frames; signal: the in-kernel cross-rank rendezvous)"""
+        sm = _shadow_maps(point_cubes, spot_maps, directional_map)
+        arr = (Image * len(out_images))(*out_images)
+        h = gbuffer.position_ao.height
+        _check(lib.vq_forward_lighting_shadowed_multi_signal(self._h, C.byref(per_frame), C.byref(per_view), C.byref(gbuffer), C.byref(env),
+                                                             C.byref(sm), arr, len(out_images), dst_row_offset, row_begin,
+                                                             h if row_end is None else row_end,
+                                                             C.byref(signal) if signal is not None else None, _stream_ptr(stream)))
+
     def depth_min_pyramid(self, depth, levels_out, n_levels=None, stream=None):
         """depth: [H,W] float32 CUDA tensor (dense rows); levels_out: flat float32 CUDA tensor of depth_pyramid_texel_count floats"""
         assert depth.dim() == 2 and depth.stride(1) == 1 and depth.element_size() == 4
@@ -389,6 +408,22 @@ class Context:
         _check(lib.vq_forward_lighting_shadowed_from_materials(self._h, C.byref(per_frame), C.byref(per_view), C.byref(inputs), table._h,
                                                                1 if alpha_mask else 0, C.byref(env), C.byref(sm), image_of(out),
                                                                row_begin, h if row_end is None else row_end, _stream_ptr(stream)))
+
+    def forward_lighting_from_materials_multi(self, per_frame, per_view, inputs: SurfaceInputs, table: "MaterialTable",
+                                              env: EnvironmentMaps, out_images, dst_row_offset, alpha_mask: bool = False, row_begin=0,
+                                              row_end=None, stream=None, point_cubes=None, spot_maps=None, directional_map=None,
+                                              signal: "PeerSignal" = None):
+        """forward_lighting_from_materials (no maps) or forward_lighting_shadowed_from_materials into several frames, as
+        forward_lighting_multi stores them; dst_row_offset must be even"""
+        bound = any(m is not None for m in (point_cubes, spot_maps, directional_map))
+        sm = _shadow_maps(point_cubes, spot_maps, directional_map) if bound else None
+        arr = (Image * len(out_images))(*out_images)
+        h = inputs.position_u.height
+        _check(lib.vq_forward_lighting_from_materials_multi_signal(self._h, C.byref(per_frame), C.byref(per_view), C.byref(inputs), table._h,
+                                                                   1 if alpha_mask else 0, C.byref(env),
+                                                                   C.byref(sm) if sm is not None else None, arr, len(out_images),
+                                                                   dst_row_offset, row_begin, h if row_end is None else row_end,
+                                                                   C.byref(signal) if signal is not None else None, _stream_ptr(stream)))
 
     # SURVEY 8(f).2: Radiance .hdr
     def hdr_decode(self, file_bytes: bytes, stream=None):

@@ -808,7 +808,7 @@ __global__ void __launch_bounds__(FWD_THREADS, FWD_CTAS_PER_SM) forward_kernel(c
 // PSMain end to end: the surface producer and K1 fused, with the G-buffer in shared memory instead of HBM
 // ---------------------------------------------------------------------------------------------
 struct PsParams {
-    FwdParams F;                       // K1's frame (outs[0] = the destination; no G-buffer planes; SHADOWED: F.shadow holds the
+    FwdParams F;                       // K1's frame (outs[0..nOut) = the destinations; no G-buffer planes; SHADOWED: F.shadow holds the
                                        // caster counts and dirSlot, its record pointer stays null)
     SurfArgs S;                        // the surface producer's inputs (no G-buffer outputs)
     vqshadow::ShadowLights L;          // SHADOWED only: what the PCF tests read besides the pixel (last, so that the unshadowed
@@ -838,7 +838,9 @@ __device__ __forceinline__ uint64_t staged_pcf_record(const vqshadow::ShadowLigh
 //             SHADOWED: first the PCF records of both pixels from the stage (all 128 threads: a warp is 32 consecutive columns of
 //             one row, as in shadow_pcf_kernel), then the shadowed light loop on them.
 // The phases stay sequential: a warp-specialised K1 measured slower (DESIGN.md §4).
-template <bool ROT, bool SHADOWED>
+// MULTI: every produced pixel goes to row dstRowOffset + y of each of the F.nOut destinations, and with a VqPeerSignal the last CTA
+// to retire runs the cross-rank rendezvous, as in forward_kernel.
+template <bool ROT, bool SHADOWED, bool MULTI = false>
 __global__ void __launch_bounds__(FWD_THREADS, FWD_CTAS_PER_SM) psmain_kernel(const __grid_constant__ PsParams Q) {
     const FwdParams& P = Q.F;
     const SurfArgs& A = Q.S;
@@ -891,8 +893,21 @@ __global__ void __launch_bounds__(FWD_THREADS, FWD_CTAS_PER_SM) psmain_kernel(co
         }
         shade_pair_lights<SHADOWED, SHADOWED>(P, s, acc, roughness, ao);
         const bool validA = inRow && sProduced[tid] != 0, validB = inRow && sProduced[FWD_THREADS + tid] != 0;
-        if (P.diffuseOnly) finish_pair<false, ROT, false>(P, sFace, s, acc, roughness, ao, y0, xA, y0 + 1, xA, validA, validB);
-        else finish_pair<false, ROT, true>(P, sFace, s, acc, roughness, ao, y0, xA, y0 + 1, xA, validA, validB);
+        if (P.diffuseOnly) finish_pair<MULTI, ROT, false>(P, sFace, s, acc, roughness, ao, y0, xA, y0 + 1, xA, validA, validB);
+        else finish_pair<MULTI, ROT, true>(P, sFace, s, acc, roughness, ao, y0, xA, y0 + 1, xA, validA, validB);
+    }
+    // forward_kernel's retirement block, copied: as a shared helper it changed the register allocation of every forward_kernel
+    if (MULTI && P.sync.n > 1) {       // fused gather: the last CTA to retire signals the peers and waits for theirs (one kernel = one step)
+        __threadfence_system();        // this CTA's peer stores are ordered before its retirement
+        __syncthreads();
+        if (tid == 0) {
+            const uint32_t done = atomicAdd(P.ticket, 1u);
+            if (done == gridDim.x * gridDim.y - 1u) {
+                *P.ticket = 0u;
+                __threadfence_system();
+                peer_rendezvous(P.sync);
+            }
+        }
     }
 }
 
@@ -1064,24 +1079,36 @@ static int frame_params(VqContext* ctx, const VqPerFrameData* pf, const VqPerVie
     return VQ_OK;
 }
 
-int vq_forward_launch_multi(VqContext* ctx, const VqPerFrameData* pf, const VqPerViewLightingData* pv,
-                            const VqGBuffer* gb, const VqEnvironmentMaps* env, const VqImage* outs, int n_outs,
-                            int dst_row_offset, int row_begin, int row_end, const VqPeerSignal* sig, cudaStream_t stream,
-                            const ShadowRecV* shadow = nullptr) {
-    VQ_REQUIRE(pf && pv && gb && env && outs, "null parameter block");
+// The destinations, row range and rendezvous of a multi-destination call over a W x H source (G-buffer or attribute planes):
+// 1..8 frames as wide as the source that hold dst_row_offset + H rows, rows inside the source, a signal only with peer
+// destinations and rows to shade (its last CTA runs the rendezvous). Host-side only; fills `sync` from `sig`.
+int vq_multi_dest_check(const VqImage* outs, int n_outs, int W, int H, int dst_row_offset, int row_begin, int row_end,
+                        const VqPeerSignal* sig, PeerSync& sync) {
     VQ_REQUIRE(n_outs >= 1 && n_outs <= 8, "1..8 destinations");
-    VQ_REQUIRE(vq_image_ok(gb->position_ao) && vq_image_ok(gb->normal_roughness) && vq_image_ok(gb->albedo_metalness), "bad image descriptor");
-    const int W = gb->position_ao.width, H = gb->position_ao.height;
-    VQ_REQUIRE(gb->normal_roughness.width == W && gb->albedo_metalness.width == W &&
-               gb->normal_roughness.height == H && gb->albedo_metalness.height == H, "G-buffer planes must have the same size");
     VQ_REQUIRE(dst_row_offset >= 0, "negative destination row offset");
     for (int k = 0; k < n_outs; ++k)
         VQ_REQUIRE(vq_image_ok(outs[k]) && outs[k].width == W && outs[k].height >= dst_row_offset + H,
                    "every destination must be as wide as the G-buffer and hold dst_row_offset + height rows");
     VQ_REQUIRE(row_begin >= 0 && row_end <= H && row_begin <= row_end, "row range out of bounds");
+    VQ_REQUIRE(row_begin < row_end || !(sig && sig->n_ranks > 1), "a rendezvous needs a non-empty row range (the kernel runs it)");
+    const int rc = vq_fill_peer_sync(sig, &sync); if (rc) return rc;
+    VQ_REQUIRE(sync.n == 0 || n_outs > 1, "a rendezvous only makes sense with peer destinations");
+    return VQ_OK;
+}
+
+int vq_forward_launch_multi(VqContext* ctx, const VqPerFrameData* pf, const VqPerViewLightingData* pv,
+                            const VqGBuffer* gb, const VqEnvironmentMaps* env, const VqImage* outs, int n_outs,
+                            int dst_row_offset, int row_begin, int row_end, const VqPeerSignal* sig, cudaStream_t stream,
+                            const ShadowRecV* shadow) {
+    VQ_REQUIRE(pf && pv && gb && env && outs, "null parameter block");
+    VQ_REQUIRE(vq_image_ok(gb->position_ao) && vq_image_ok(gb->normal_roughness) && vq_image_ok(gb->albedo_metalness), "bad image descriptor");
+    const int W = gb->position_ao.width, H = gb->position_ao.height;
+    VQ_REQUIRE(gb->normal_roughness.width == W && gb->albedo_metalness.width == W &&
+               gb->normal_roughness.height == H && gb->albedo_metalness.height == H, "G-buffer planes must have the same size");
+    PeerSync sync;
+    int rc = vq_multi_dest_check(outs, n_outs, W, H, dst_row_offset, row_begin, row_end, sig, sync); if (rc) return rc;
     const VqSceneLighting& L = pf->Lights;
     VQ_REQUIRE(light_counts_ok(L), "light counts exceed the cbuffer arrays");
-    VQ_REQUIRE(row_begin < row_end || !(sig && sig->n_ranks > 1), "a rendezvous needs a non-empty row range (the kernel runs it)");
     if (row_begin == row_end) return VQ_OK;
     VqScratchLock lock(ctx);           // the registered environment and the per-call sampling copies are the context's
 
@@ -1095,18 +1122,16 @@ int vq_forward_launch_multi(VqContext* ctx, const VqPerFrameData* pf, const VqPe
         VQ_REQUIRE(vq_image_ok(gb->emissive) && gb->emissive.width == W && gb->emissive.height == H, "bad emissive plane");
         P.emi = make_view(gb->emissive);
     }
-    int rc = frame_params(ctx, pf, pv, env, stream, P); if (rc) return rc;
+    rc = frame_params(ctx, pf, pv, env, stream, P); if (rc) return rc;
     P.rowBegin = row_begin; P.rows = row_end - row_begin; P.width = W;
     const bool shadowed = shadow && shadow->p;
     if (shadowed) {
-        VQ_REQUIRE(n_outs == 1, "the shadowed pass writes one destination");
         VQ_REQUIRE(shadow->nPointCasters == L.numPointCasters && shadow->nSpotCasters == L.numSpotCasters && shadow->pitch >= W,
                    "PCF records do not match the frame's caster lists");
         P.shadow = *shadow;
     }
 
-    rc = vq_fill_peer_sync(sig, &P.sync); if (rc) return rc;
-    VQ_REQUIRE(P.sync.n == 0 || n_outs > 1, "a rendezvous only makes sense with peer destinations");
+    P.sync = sync;
     P.ticket = P.sync.n > 1 ? vq_ticket_pair(ctx) : nullptr;
 
     // persistent grid: x = the row's 256-pixel tiles, y = row groups striding the rows
@@ -1126,6 +1151,8 @@ int vq_forward_launch_multi(VqContext* ctx, const VqPerFrameData* pf, const VqPe
         VQ_CUDA_OK(cudaFuncSetAttribute(forward_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
         VQ_CUDA_OK(cudaFuncSetAttribute(forward_kernel<false, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
         VQ_CUDA_OK(cudaFuncSetAttribute(forward_kernel<false, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
+        VQ_CUDA_OK(cudaFuncSetAttribute(forward_kernel<true, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
+        VQ_CUDA_OK(cudaFuncSetAttribute(forward_kernel<true, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
         attrSet.store(true, std::memory_order_release);
     }
     auto launch = [&](auto kernel) -> int {
@@ -1136,7 +1163,8 @@ int vq_forward_launch_multi(VqContext* ctx, const VqPerFrameData* pf, const VqPe
         return VQ_OK;
     };
     VQ_REQUIRE(smem <= 96 * 1024, "stage layout exceeds the shared-memory budget");
-    if (shadowed) rc = rot ? launch(forward_kernel<false, true, true>) : launch(forward_kernel<false, false, true>);
+    if (shadowed && n_outs > 1) rc = rot ? launch(forward_kernel<true, true, true>) : launch(forward_kernel<true, false, true>);
+    else if (shadowed) rc = rot ? launch(forward_kernel<false, true, true>) : launch(forward_kernel<false, false, true>);
     else if (n_outs > 1) rc = rot ? launch(forward_kernel<true, true>) : launch(forward_kernel<true, false>);
     else rc = rot ? launch(forward_kernel<false, true>) : launch(forward_kernel<false, false>);
     if (rc) return rc;
@@ -1176,18 +1204,26 @@ extern "C" int vq_forward_lighting_multi_signal(VqContext* ctx, const VqPerFrame
 }
 
 // PSMain from interpolants and materials in one launch (psmain_kernel): what vq_gbuffer_from_materials with an emissive plane
-// followed by vq_forward_lighting (sm == nullptr) or vq_forward_lighting_shadowed computes, without the G-buffer. The arguments are
-// checked before the device is touched.
+// followed by vq_forward_lighting (sm == nullptr) or vq_forward_lighting_shadowed computes, without the G-buffer. `multi`: the
+// multi-destination call (outs[0..n_outs), rows offset by dst_row_offset, optional rendezvous); otherwise outs[0] is the one output,
+// of the attribute planes' size. The arguments are checked before the device is touched.
 static int psmain_launch(VqContext* ctx, const VqPerFrameData* pf, const VqPerViewLightingData* pv, const VqSurfaceInputs* in,
                          const VqMaterialTable* table, int alpha_mask, const VqEnvironmentMaps* env, const VqShadowMaps* sm,
-                         VqImage out, int row_begin, int row_end, void* stream) {
-    VQ_REQUIRE(pf && pv && env && in, "null argument");
+                         bool multi, const VqImage* outs, int n_outs, int dst_row_offset, int row_begin, int row_end,
+                         const VqPeerSignal* sig, void* stream) {
+    VQ_REQUIRE(pf && pv && env && in && outs, "null argument");
     const int W = in->position_u.width, H = in->position_u.height;
-    VQ_REQUIRE(vq_image_ok(out) && out.width == W && out.height == H, "the output must have the size of the attribute planes");
     static_assert(sizeof(PsParams) <= 32764, "kernel parameter space");
     PsParams Q;
     memset(&Q, 0, sizeof(Q));
     int rc;
+    if (multi) {
+        rc = vq_multi_dest_check(outs, n_outs, W, H, dst_row_offset, row_begin, row_end, sig, Q.F.sync); if (rc) return rc;
+        // the surface producer's quads sit on even rows of the attribute planes: an even offset keeps them on even rows of the frame
+        VQ_REQUIRE((dst_row_offset & 1) == 0, "dst_row_offset must be even (quads are aligned to even rows)");
+    } else {
+        VQ_REQUIRE(vq_image_ok(outs[0]) && outs[0].width == W && outs[0].height == H, "the output must have the size of the attribute planes");
+    }
     bool shadowed = false;                                        // does any PCF test run?
     if (sm) {
         rc = vq_shadow_maps_check(pf->Lights, *sm); if (rc) return rc;
@@ -1203,7 +1239,9 @@ static int psmain_launch(VqContext* ctx, const VqPerFrameData* pf, const VqPerVi
     FwdParams& P = Q.F;
     rc = frame_params(ctx, pf, pv, env, (cudaStream_t)stream, P); if (rc) return rc;
     P.hasEmissive = 1;
-    P.outs[0] = make_view(out); P.nOut = 1;
+    for (int k = 0; k < n_outs; ++k) P.outs[k] = make_view(outs[k]);
+    P.nOut = n_outs; P.dstRowOffset = dst_row_offset;
+    P.ticket = P.sync.n > 1 ? vq_ticket_pair(ctx) : nullptr;
     P.rowBegin = row_begin; P.rows = row_end - row_begin; P.width = W;
     // persistent grid: x = the row's 128-column tiles, y = groups striding the row pairs
     const unsigned gx = (unsigned)((W + FWD_THREADS - 1) / FWD_THREADS);
@@ -1212,22 +1250,20 @@ static int psmain_launch(VqContext* ctx, const VqPerFrameData* pf, const VqPerVi
     if (gy < 1) gy = 1;
     if (gy > pairs) gy = pairs;
     const bool rot = P.sinB != 0.0f || P.cosB != 1.0f;
-    const dim3 grid(gx, gy);
-    const cudaStream_t s = (cudaStream_t)stream;
-    if (shadowed) {
-        if (rot) psmain_kernel<true, true><<<grid, FWD_THREADS, 0, s>>>(Q);
-        else psmain_kernel<false, true><<<grid, FWD_THREADS, 0, s>>>(Q);
-    } else {
-        if (rot) psmain_kernel<true, false><<<grid, FWD_THREADS, 0, s>>>(Q);
-        else psmain_kernel<false, false><<<grid, FWD_THREADS, 0, s>>>(Q);
-    }
-    return vq_check_launch(sm ? "forward_lighting_shadowed_from_materials" : "forward_lighting_from_materials");
+    void (*kernel)(PsParams);          // one destination: the single-destination kernels, as vq_forward_launch_multi picks them
+    if (shadowed) kernel = n_outs > 1 ? (rot ? psmain_kernel<true, true, true> : psmain_kernel<false, true, true>)
+                                      : (rot ? psmain_kernel<true, true> : psmain_kernel<false, true>);
+    else kernel = n_outs > 1 ? (rot ? psmain_kernel<true, false, true> : psmain_kernel<false, false, true>)
+                             : (rot ? psmain_kernel<true, false> : psmain_kernel<false, false>);
+    kernel<<<dim3(gx, gy), FWD_THREADS, 0, (cudaStream_t)stream>>>(Q);
+    return vq_check_launch(multi ? "forward_lighting_from_materials_multi"
+                                 : sm ? "forward_lighting_shadowed_from_materials" : "forward_lighting_from_materials");
 }
 
 extern "C" int vq_forward_lighting_from_materials(VqContext* ctx, const VqPerFrameData* pf, const VqPerViewLightingData* pv,
                                                   const VqSurfaceInputs* in, const VqMaterialTable* table, int alpha_mask,
                                                   const VqEnvironmentMaps* env, VqImage out, int row_begin, int row_end, void* stream) {
-    return psmain_launch(ctx, pf, pv, in, table, alpha_mask, env, nullptr, out, row_begin, row_end, stream);
+    return psmain_launch(ctx, pf, pv, in, table, alpha_mask, env, nullptr, false, &out, 1, 0, row_begin, row_end, nullptr, stream);
 }
 
 // The same with the shadow maps bound: the PCF tests run inside psmain_kernel on the staged positions and normals, so there are no
@@ -1237,7 +1273,18 @@ extern "C" int vq_forward_lighting_shadowed_from_materials(VqContext* ctx, const
                                                            const VqEnvironmentMaps* env, const VqShadowMaps* sm, VqImage out,
                                                            int row_begin, int row_end, void* stream) {
     VQ_REQUIRE(sm, "null shadow maps");
-    return psmain_launch(ctx, pf, pv, in, table, alpha_mask, env, sm, out, row_begin, row_end, stream);
+    return psmain_launch(ctx, pf, pv, in, table, alpha_mask, env, sm, false, &out, 1, 0, row_begin, row_end, nullptr, stream);
+}
+
+// Both with every pixel stored into each of n_outs frames at row dst_row_offset + y and the optional rendezvous (shadow_maps NULL:
+// unshadowed), as vq_forward_lighting_multi_signal does for the G-buffer pass.
+extern "C" int vq_forward_lighting_from_materials_multi_signal(VqContext* ctx, const VqPerFrameData* pf, const VqPerViewLightingData* pv,
+                                                               const VqSurfaceInputs* in, const VqMaterialTable* table, int alpha_mask,
+                                                               const VqEnvironmentMaps* env, const VqShadowMaps* sm, const VqImage* outs,
+                                                               int n_outs, int dst_row_offset, int row_begin, int row_end,
+                                                               const VqPeerSignal* signal, void* stream) {
+    return psmain_launch(ctx, pf, pv, in, table, alpha_mask, env, sm, true, outs, n_outs, dst_row_offset, row_begin, row_end, signal,
+                         stream);
 }
 
 // The IBL cubemaps and the BRDF LUT are sampled from footprint-friendly copies (see CubeV, LutV).

@@ -148,18 +148,15 @@ bool vq_shadow_slots(const VqSceneLighting& L, const VqShadowMaps& sm, vq::Shado
     return (sm.point_cubes && L.numPointCasters > 0) || (sm.spot_maps && L.numSpotCasters > 0) || dirTest;
 }
 
-extern "C" int vq_forward_lighting_shadowed(VqContext* ctx, const VqPerFrameData* pf, const VqPerViewLightingData* pv,
-                                            const VqGBuffer* gb, const VqEnvironmentMaps* env, const VqShadowMaps* sm,
-                                            VqImage out, int row_begin, int row_end, void* stream) {
-    int rc = vq_enter(ctx); if (rc) return rc;
-    VQ_MARK("RenderSceneColor");
-    VQ_REQUIRE(pf && pv && gb && env && sm, "null parameter block");
-    const VqSceneLighting& L = pf->Lights;
-    rc = vq_shadow_maps_check(L, *sm); if (rc) return rc;
+// The PCF kernel over rows [row_begin, row_end) of the G-buffer, then the shadowed forward pass into outs[0..n_outs) (rows offset by
+// dst_row_offset, optional rendezvous); when no test runs, the plain forward pass. The shadow maps have been checked.
+static int shadowed_passes(VqContext* ctx, const VqPerFrameData* pf, const VqPerViewLightingData* pv, const VqGBuffer* gb,
+                           const VqEnvironmentMaps* env, const VqShadowMaps& sm, const VqImage* outs, int n_outs, int dst_row_offset,
+                           int row_begin, int row_end, const VqPeerSignal* sig, cudaStream_t stream) {
     vq::ShadowRecV V;
-    const bool anyTest = vq_shadow_slots(L, *sm, V);
+    const bool anyTest = vq_shadow_slots(pf->Lights, sm, V);
     if (!anyTest || row_begin >= row_end)          // no test runs: every factor is 1, which is what the plain kernel computes
-        return vq_forward_launch(ctx, pf, pv, gb, env, out, row_begin, row_end, (cudaStream_t)stream);
+        return vq_forward_launch_multi(ctx, pf, pv, gb, env, outs, n_outs, dst_row_offset, row_begin, row_end, sig, stream);
     VQ_REQUIRE(gb->position_ao.ptr && vq_image_ok(gb->position_ao) && vq_image_ok(gb->normal_roughness) &&
                gb->normal_roughness.width == gb->position_ao.width && gb->normal_roughness.height == gb->position_ao.height,
                "bad G-buffer planes");
@@ -169,9 +166,9 @@ extern "C" int vq_forward_lighting_shadowed(VqContext* ctx, const VqPerFrameData
     memset(&P, 0, sizeof(P));
     P.pos = make_view(gb->position_ao); P.nrm = make_view(gb->normal_roughness);
     P.rowBegin = row_begin; P.rows = row_end - row_begin; P.width = gb->position_ao.width;
-    vqshadow::fill_shadow_lights(P.L, *pf, *pv, *sm);
+    vqshadow::fill_shadow_lights(P.L, *pf, *pv, sm);
     VqScratchLock lock(ctx);                       // the records are context scratch (vqcuda.h lists the call as not re-entrant per context)
-    rc = vq_scratch_reserve(ctx->shadow_rec, (size_t)P.width * P.rows * sizeof(uint2), "PCF records"); if (rc) return rc;
+    int rc = vq_scratch_reserve(ctx->shadow_rec, (size_t)P.width * P.rows * sizeof(uint2), "PCF records"); if (rc) return rc;
     P.rec = (uint2*)ctx->shadow_rec.p; P.recPitch = P.width;
 
     const unsigned gx = (unsigned)((P.width + 127) / 128);
@@ -179,11 +176,43 @@ extern "C" int vq_forward_lighting_shadowed(VqContext* ctx, const VqPerFrameData
     if (gy < 1) gy = 1;
     if (gy > (unsigned)P.rows) gy = (unsigned)P.rows;
     if (gy > 65535u) gy = 65535u;
-    shadow_pcf_kernel<<<dim3(gx, gy), 128, 0, (cudaStream_t)stream>>>(P);
+    shadow_pcf_kernel<<<dim3(gx, gy), 128, 0, stream>>>(P);
     rc = vq_check_launch("shadow_pcf"); if (rc) return rc;
 
     V.p = P.rec; V.pitch = P.recPitch;
-    return vq_forward_launch(ctx, pf, pv, gb, env, out, row_begin, row_end, (cudaStream_t)stream, &V);
+    return vq_forward_launch_multi(ctx, pf, pv, gb, env, outs, n_outs, dst_row_offset, row_begin, row_end, sig, stream, &V);
+}
+
+extern "C" int vq_forward_lighting_shadowed(VqContext* ctx, const VqPerFrameData* pf, const VqPerViewLightingData* pv,
+                                            const VqGBuffer* gb, const VqEnvironmentMaps* env, const VqShadowMaps* sm,
+                                            VqImage out, int row_begin, int row_end, void* stream) {
+    int rc = vq_enter(ctx); if (rc) return rc;
+    VQ_MARK("RenderSceneColor");
+    VQ_REQUIRE(pf && pv && gb && env && sm, "null parameter block");
+    rc = vq_shadow_maps_check(pf->Lights, *sm); if (rc) return rc;
+    VQ_REQUIRE(vq_image_ok(out) && out.height == gb->position_ao.height, "G-buffer planes and output must have the same size");
+    return shadowed_passes(ctx, pf, pv, gb, env, *sm, &out, 1, 0, row_begin, row_end, nullptr, (cudaStream_t)stream);
+}
+
+// The same into n_outs frames (vq_forward_lighting_multi_signal's destinations, row offset and rendezvous). The shadow maps, the
+// G-buffer, the destinations, the row range and the signal are checked before the device is touched.
+extern "C" int vq_forward_lighting_shadowed_multi_signal(VqContext* ctx, const VqPerFrameData* pf, const VqPerViewLightingData* pv,
+                                                         const VqGBuffer* gb, const VqEnvironmentMaps* env, const VqShadowMaps* sm,
+                                                         const VqImage* outs, int n_outs, int dst_row_offset, int row_begin, int row_end,
+                                                         const VqPeerSignal* signal, void* stream) {
+    VQ_REQUIRE(pf && pv && gb && env && sm && outs, "null parameter block");
+    int rc = vq_shadow_maps_check(pf->Lights, *sm); if (rc) return rc;
+    VQ_REQUIRE(vq_image_ok(gb->position_ao) && vq_image_ok(gb->normal_roughness) && vq_image_ok(gb->albedo_metalness), "bad image descriptor");
+    const int W = gb->position_ao.width, H = gb->position_ao.height;
+    VQ_REQUIRE(gb->normal_roughness.width == W && gb->albedo_metalness.width == W &&
+               gb->normal_roughness.height == H && gb->albedo_metalness.height == H, "G-buffer planes must have the same size");
+    if (gb->emissive.ptr)
+        VQ_REQUIRE(vq_image_ok(gb->emissive) && gb->emissive.width == W && gb->emissive.height == H, "bad emissive plane");
+    PeerSync sync;
+    rc = vq_multi_dest_check(outs, n_outs, W, H, dst_row_offset, row_begin, row_end, signal, sync); if (rc) return rc;
+    rc = vq_enter(ctx); if (rc) return rc;
+    VQ_MARK("RenderSceneColor");
+    return shadowed_passes(ctx, pf, pv, gb, env, *sm, outs, n_outs, dst_row_offset, row_begin, row_end, signal, (cudaStream_t)stream);
 }
 
 extern "C" int vq_depth_pyramid_level_count(int width, int height) { return vqshadow::depth_level_count(width, height); }

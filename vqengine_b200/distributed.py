@@ -24,6 +24,15 @@ def equal_tiles(n_rows: int, world: int) -> List[Tuple[int, int]]:
     return [((n_rows * r) // world, (n_rows * (r + 1)) // world) for r in range(world)]
 
 
+def even_tiles(n_rows: int, world: int) -> List[Tuple[int, int]]:
+    """`world` contiguous [begin,end) row ranges whose inner boundaries are even rows and whose sizes differ by at most two (some
+    may be empty): the bands of the from-materials shading calls, whose 2x2 quads must start on even rows of the frame. Row pairs
+    are shared out with the larger shares first, so that an odd last row goes to a band of the smaller size."""
+    pairs = n_rows // 2
+    cuts = [2 * (-(-pairs * r // world)) for r in range(world)] + [n_rows]
+    return [(cuts[r], cuts[r + 1]) for r in range(world)]
+
+
 def weighted_tiles(costs: Sequence[float], world: int) -> List[Tuple[int, int]]:
     """contiguous ranges over rows with per-row `costs`, cut where the cumulative cost crosses k/world."""
     total = float(sum(costs))
