@@ -318,6 +318,29 @@ VQ_API int vq_fsr_easu(VqContext* ctx, const uint32_t easu_const[16], int addres
 VQ_API int vq_fsr_rcas(VqContext* ctx, const uint32_t rcas_const[4], VqImage in, VqImage out, void* stream);
 
 /* ------------------------------------------------------------------------------------------
+ * K6-K9 on a band of the output, into several frames: one rank's share of the post chain of a multi-GPU frame
+ * (DESIGN.md §6). `in` is the pass's whole source image (the stencils read across band edges); rows [row_begin,row_end) are
+ * rows of the pass's output; each of the n_outs (1..8) destinations has the output's size (the tonemapper's, CAS's and RCAS's
+ * output is the size of `in`; EASU's is the size of outs[0]). Into each destination the call stores exactly the bits its
+ * single-destination call (vq_tonemap, vq_cas, vq_fsr_easu, vq_fsr_rcas) stores on those rows, and touches no other row of any
+ * destination. One launch per call, no context scratch: calls on several streams of one context are fine. With `signal`
+ * (n_ranks > 1) the kernel's last CTA runs the rendezvous of VqPeerSignal after every store; NULL: no rendezvous. An empty row
+ * range without a rendezvous launches nothing and returns VQ_OK.
+ * Refused with VQ_ERR_INVALID_ARG before the device is touched (also with a NULL context): the single call's checks and messages
+ * (null constants or params, size rules, `in` equal to any destination for CAS / EASU / RCAS, EASU's con0 checks above and an
+ * unknown address mode), n_outs outside 1..8, rows outside the output or reversed, a signal with n_ranks > 1 and one
+ * destination or an empty row range.
+ * ------------------------------------------------------------------------------------------ */
+VQ_API int vq_tonemap_multi_signal(VqContext* ctx, const VqTonemapperParams* params, VqImage in, const VqImage* outs, int n_outs,
+                                   int row_begin, int row_end, const VqPeerSignal* signal, void* stream);
+VQ_API int vq_cas_multi_signal(VqContext* ctx, const uint32_t cas_const[8], VqImage in, const VqImage* outs, int n_outs,
+                               int row_begin, int row_end, const VqPeerSignal* signal, void* stream);
+VQ_API int vq_fsr_easu_multi_signal(VqContext* ctx, const uint32_t easu_const[16], int address_mode, VqImage in, const VqImage* outs,
+                                    int n_outs, int row_begin, int row_end, const VqPeerSignal* signal, void* stream);
+VQ_API int vq_fsr_rcas_multi_signal(VqContext* ctx, const uint32_t rcas_const[4], VqImage in, const VqImage* outs, int n_outs,
+                                    int row_begin, int row_end, const VqPeerSignal* signal, void* stream);
+
+/* ------------------------------------------------------------------------------------------
  * K10 FidelityFX SPD: the whole mip chain in one launch.  Replaces SPD_CSMain
  *     (AMDFidelityFX.hlsl:525-545) -> SpdDownsample (SPD/ffx_spd.h:811-835), reduction =
  *     (v0+v1+v2+v3)*0.25 (AMDFidelityFX.hlsl:463-466). `mips` are the destination levels
@@ -335,6 +358,14 @@ VQ_API void vq_fsr_easu_con(uint32_t con[16],
                             float input_viewport_w, float input_viewport_h,
                             float input_size_w, float input_size_h,
                             float output_w, float output_h);
+/* HOST. The rows of `in` that vq_fsr_easu reads for output rows [row_begin,row_end): up to two increasing, disjoint, non-adjacent
+ * [begin,end) ranges in ranges[0..3]; returns their count (0 for an empty range) or VQ_ERR_INVALID_ARG (null pointers, unknown
+ * address mode, heights < 1, rows outside the output or reversed, con0.y / con0.w not finite or putting taps outside [-H, 2H)).
+ * The taps of output row y are the rows floor(y * con0.y + con0.w) - 1 .. + 2 folded by the address mode; under WRAP the first
+ * and last bands of an upscale also read rows at the opposite edge, hence the second range. Exact whenever consecutive output
+ * rows move at most 4 input rows (con0.y <= 4, every vq_fsr_easu_con with output >= input / 4); a covering superset otherwise. */
+VQ_API int vq_fsr_easu_source_rows(const uint32_t easu_const[16], int address_mode, int in_height, int out_height,
+                                   int row_begin, int row_end, int ranges[4]);
 /* FsrRcasCon (ffx_fsr1.h:662-672) */
 VQ_API void vq_fsr_rcas_con(uint32_t con[4], float sharpness_stops);
 /* CasSetup (ffx_cas.h:375-394) -> con[8] = const0|const1 */

@@ -36,6 +36,8 @@ ABI_SYMBOLS = [
     "vq_forward_lighting_shadowed", "vq_depth_pyramid_level_count", "vq_depth_pyramid_texel_count", "vq_depth_min_pyramid",
     "vq_forward_lighting_from_materials", "vq_forward_lighting_shadowed_from_materials",
     "vq_forward_lighting_shadowed_multi_signal", "vq_forward_lighting_from_materials_multi_signal",
+    "vq_tonemap_multi_signal", "vq_cas_multi_signal", "vq_fsr_easu_multi_signal", "vq_fsr_rcas_multi_signal",
+    "vq_fsr_easu_source_rows",
 ]
 
 
@@ -82,6 +84,11 @@ def _load() -> C.CDLL:
     lib.vq_fsr_easu.argtypes = [vp, P(u32), C.c_int, Image, Image, vp]
     lib.vq_fsr_rcas.argtypes = [vp, P(u32), Image, Image, vp]
     lib.vq_spd_downsample.argtypes = [vp, P(SpdConstants), Image, P(Image), vp]
+    lib.vq_tonemap_multi_signal.argtypes = [vp, P(TonemapperParams), Image, P(Image), C.c_int, C.c_int, C.c_int, P(PeerSignal), vp]
+    lib.vq_cas_multi_signal.argtypes = [vp, P(u32), Image, P(Image), C.c_int, C.c_int, C.c_int, P(PeerSignal), vp]
+    lib.vq_fsr_easu_multi_signal.argtypes = [vp, P(u32), C.c_int, Image, P(Image), C.c_int, C.c_int, C.c_int, P(PeerSignal), vp]
+    lib.vq_fsr_rcas_multi_signal.argtypes = [vp, P(u32), Image, P(Image), C.c_int, C.c_int, C.c_int, P(PeerSignal), vp]
+    lib.vq_fsr_easu_source_rows.argtypes = [P(u32), C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, P(C.c_int)]
     lib.vq_fsr_easu_con.argtypes = [P(u32), f32, f32, f32, f32, f32, f32]
     lib.vq_fsr_easu_con.restype = None
     lib.vq_fsr_rcas_con.argtypes = [P(u32), f32]
@@ -146,6 +153,15 @@ def fsr_easu_con(vp_w, vp_h, in_w, in_h, out_w, out_h):
     con = (u32 * 16)()
     lib.vq_fsr_easu_con(con, vp_w, vp_h, in_w, in_h, out_w, out_h)
     return con
+
+
+def fsr_easu_source_rows(con, in_h: int, out_h: int, row_begin: int, row_end: int, address_mode=VQ_ADDRESS_WRAP):
+    """the rows of the input vq_fsr_easu reads for output rows [row_begin, row_end): a list of up to two [begin, end) ranges"""
+    r = (C.c_int * 4)()
+    n = lib.vq_fsr_easu_source_rows(con, address_mode, in_h, out_h, row_begin, row_end, r)
+    if n < 0:
+        _check(n)
+    return [(r[2 * i], r[2 * i + 1]) for i in range(n)]
 
 
 def fsr_rcas_con(stops: float):
@@ -539,6 +555,26 @@ class Context:
 
     def fsr_rcas(self, con, src, dst, stream=None):
         _check(lib.vq_fsr_rcas(self._h, con, image_of(src), image_of(dst), _stream_ptr(stream)))
+
+    # one rank's band of a post pass into several frames (vq_*_multi_signal): src is the pass's whole source tensor, out_images the
+    # Image descriptors of the destinations (the local frame first, then the peers' mapped frames), rows are rows of the output
+    def _post_multi(self, fn, args, src, out_images, row_begin, row_end, stream, signal):
+        arr = (Image * max(len(out_images), 1))(*out_images)
+        re = (out_images[0].height if out_images else 0) if row_end is None else row_end
+        _check(fn(self._h, *args, image_of(src), arr, len(out_images), row_begin, re,
+                  C.byref(signal) if signal is not None else None, _stream_ptr(stream)))
+
+    def tonemap_multi(self, params: TonemapperParams, src, out_images, row_begin=0, row_end=None, stream=None, signal=None):
+        self._post_multi(lib.vq_tonemap_multi_signal, (C.byref(params),), src, out_images, row_begin, row_end, stream, signal)
+
+    def cas_multi(self, con, src, out_images, row_begin=0, row_end=None, stream=None, signal=None):
+        self._post_multi(lib.vq_cas_multi_signal, (con,), src, out_images, row_begin, row_end, stream, signal)
+
+    def fsr_easu_multi(self, con, src, out_images, row_begin=0, row_end=None, address_mode=VQ_ADDRESS_WRAP, stream=None, signal=None):
+        self._post_multi(lib.vq_fsr_easu_multi_signal, (con, address_mode), src, out_images, row_begin, row_end, stream, signal)
+
+    def fsr_rcas_multi(self, con, src, out_images, row_begin=0, row_end=None, stream=None, signal=None):
+        self._post_multi(lib.vq_fsr_rcas_multi_signal, (con,), src, out_images, row_begin, row_end, stream, signal)
 
     def spd_downsample(self, constants: SpdConstants, src, mips, stream=None):
         arr = (Image * len(mips))(*[image_of(m) for m in mips])

@@ -68,4 +68,29 @@ inline Verdict check(const float c[4], int in_w, int in_h, int out_w, int out_h,
     return nx <= UP_TILE_X && ny <= UP_TILE_Y ? EASU_OK : EASU_TILE_FOOTPRINT;
 }
 
+// The input rows the kernels read for output rows [rb, re) of an axis that axis_ok accepts: the taps f-1 .. f+2 of every
+// 'f' = floor(pos(y)), folded into [0, n_in) as load_addr folds them (wrap: modulo n_in; otherwise clamped), as up to two
+// increasing, disjoint, non-adjacent [begin, end) ranges in r[0..3]. Returns their count (0 for an empty range).
+// 'f' is monotone in y, so the taps span [min f - 1, max f + 2] with f at rb and re - 1; every row of that span is read when
+// consecutive outputs' 'f' differ by at most 4 (|scale| <= 4: every FsrEasuCon with output >= input / 4), a superset otherwise.
+// Under wrap a span shorter than the image folds into at most two pieces: the top band of a 2x upscale also reads the last
+// input rows, the bottom band the first ones.
+inline int source_rows(float scale, float bias, bool wrap, int n_in, int rb, int re, int r[4]) {
+    if (rb >= re) return 0;
+    const int fa = (int)floorf(pos(rb, scale, bias)), fb = (int)floorf(pos(re - 1, scale, bias));
+    int lo = (fa < fb ? fa : fb) - 1, hi = (fa < fb ? fb : fa) + 2;          // inclusive, unfolded
+    if (!wrap) {
+        lo = lo < 0 ? 0 : (lo > n_in - 1 ? n_in - 1 : lo);
+        hi = hi < 0 ? 0 : (hi > n_in - 1 ? n_in - 1 : hi);
+        r[0] = lo; r[1] = hi + 1;
+        return 1;
+    }
+    if (hi - lo + 1 >= n_in) { r[0] = 0; r[1] = n_in; return 1; }
+    const int a = (lo % n_in + n_in) % n_in, b = a + (hi - lo);             // folded start; end before the second fold
+    if (b < n_in) { r[0] = a; r[1] = b + 1; return 1; }
+    r[0] = 0; r[1] = b - n_in + 1;                                          // < a: the span is shorter than the image
+    r[2] = a; r[3] = n_in;
+    return 2;
+}
+
 }  // namespace vqeasu

@@ -7,8 +7,60 @@
 // kernel); parity against oracle/ is tested in tests/test_post_gpu.py.
 #include "vq_common.cuh"
 #include "vq_easu_check.cuh"
+#include <string.h>
+#include <algorithm>
+#include <type_traits>
 
 using namespace vq;
+
+// =============================================================================================
+// Multi-destination form of K6-K9 (vq_*_multi_signal): the MULTI instantiation of a kernel takes a PostDests where the
+// single-destination one takes its output view. It keeps the full-frame tile grid, launched only over the tile rows that meet
+// [rowBegin, rowEnd) (tile row = blockIdx.y + by0), so every pixel is computed from the same staged values as in the full-frame
+// launch; stores are masked to the range and go to each of the n frames. With a rendezvous (sync.n > 1) the last CTA to retire
+// runs it, as forward_kernel<MULTI> does.
+// =============================================================================================
+struct PostDests {
+    ImgV o[8];
+    int n, w, h;                       // destinations, and the output's size (every destination has it)
+    int rowBegin, rowEnd, by0;
+    PeerSync sync;
+    uint32_t* ticket;                  // retired-CTA count (zero between launches); sync.n > 1 only
+};
+template <bool MULTI> using PostOut = typename std::conditional<MULTI, PostDests, ImgV>::type;
+
+__device__ __forceinline__ unsigned tile_row(const ImgV&) { return blockIdx.y; }
+__device__ __forceinline__ unsigned tile_row(const PostDests& d) { return blockIdx.y + (unsigned)d.by0; }
+__device__ __forceinline__ void store_px(const ImgV& o, int x, int y, float4 v) { st_stream(o.row(y) + x, v); }
+__device__ __forceinline__ void store_px(const PostDests& d, int x, int y, float4 v) {
+    if (y < d.rowBegin || y >= d.rowEnd) return;
+#pragma unroll
+    for (int q = 0; q < 8; ++q)        // constant indices: the views stay in the parameter bank
+        if (q < d.n) st_stream(d.o[q].row(y) + x, v);
+}
+// Kernels that compute their output row pointer once store with store_px(out, out_row(out, y) + x, x, y, v): the
+// single-destination instantiation stores to that address (the code it had before MULTI existed), MULTI to (x, y) of every
+// destination.
+__device__ __forceinline__ float4* out_row(const ImgV& o, int y) { return o.row(y); }
+__device__ __forceinline__ float4* out_row(const PostDests& d, int y) { return d.o[0].row(y); }
+__device__ __forceinline__ void store_px(const ImgV&, float4* p, int, int, float4 v) { st_stream(p, v); }
+__device__ __forceinline__ void store_px(const PostDests& d, float4*, int x, int y, float4 v) { store_px(d, x, y, v); }
+// Every thread of the CTA calls it once: after its last store, or where it leaves early. The barrier is the non-aligned
+// barrier.sync, which threads may reach from different places in the kernel.
+__device__ __forceinline__ void post_retire(const ImgV&) {}
+__device__ __forceinline__ void post_retire(const PostDests& d) {
+    if (d.sync.n <= 1) return;
+    __threadfence_system();            // this thread's peer stores are ordered before the CTA's retirement
+    asm volatile("barrier.sync 0;" ::: "memory");
+    if (threadIdx.x == 0 && threadIdx.y == 0) {
+        const uint32_t done = atomicAdd(d.ticket, 1u);
+        if (done == gridDim.x * gridDim.y - 1u) {
+            *d.ticket = 0u;
+            __threadfence_system();
+            peer_rendezvous(d.sync);
+        }
+    }
+}
 
 // =============================================================================================
 // K6 Tonemapper — Shaders/Tonemapper.hlsl:110-151, Shaders/HDR.hlsl:76-119
@@ -53,12 +105,12 @@ __device__ __forceinline__ float4 tonemap_px(float4 in, float hdrScalar) {
 constexpr int TM_THREADS = 256;
 constexpr int TM_PX = 4;   // pixels per thread, loads issued back to back for memory-level parallelism
 
-template <int CURVE, bool GAMMA, bool TO2020>
-__global__ void __launch_bounds__(TM_THREADS) tonemap_kernel(ImgV in, ImgV out, float hdrScalar) {
-    const int y = blockIdx.y;
+template <int CURVE, bool GAMMA, bool TO2020, bool MULTI = false>
+__global__ void __launch_bounds__(TM_THREADS) tonemap_kernel(ImgV in, PostOut<MULTI> out, float hdrScalar) {
+    const int y = tile_row(out);
     const int x0 = blockIdx.x * (TM_THREADS * TM_PX) + threadIdx.x;
     const float4* __restrict__ src = in.row(y);
-    float4* __restrict__ dst = out.row(y);
+    float4* __restrict__ dst = out_row(out, y);
     float4 v[TM_PX];
 #pragma unroll
     for (int i = 0; i < TM_PX; ++i) {
@@ -68,7 +120,29 @@ __global__ void __launch_bounds__(TM_THREADS) tonemap_kernel(ImgV in, ImgV out, 
 #pragma unroll
     for (int i = 0; i < TM_PX; ++i) {
         const int x = x0 + i * TM_THREADS;
-        if (x < in.w) st_stream(dst + x, tonemap_px<CURVE, GAMMA, TO2020>(v[i], hdrScalar));
+        if (x < in.w) store_px(out, dst + x, x, y, tonemap_px<CURVE, GAMMA, TO2020>(v[i], hdrScalar));
+    }
+    post_retire(out);
+}
+
+template <bool MULTI>
+static void tonemap_launch(const VqTonemapperParams* p, dim3 grid, ImgV vi, const PostOut<MULTI>& vo, cudaStream_t s) {
+    const float hdrScalar = p->DisplayReferenceBrightnessLevel / 10000.0f;   // ST2084_MAX, HDR.hlsl:43
+    switch (p->OutputDisplayCurve) {
+        case VQ_DISPLAY_CURVE_SRGB:
+            if (p->ToggleGammaCorrection) tonemap_kernel<VQ_DISPLAY_CURVE_SRGB, true, false, MULTI><<<grid, TM_THREADS, 0, s>>>(vi, vo, hdrScalar);
+            else                          tonemap_kernel<VQ_DISPLAY_CURVE_SRGB, false, false, MULTI><<<grid, TM_THREADS, 0, s>>>(vi, vo, hdrScalar);
+            break;
+        case VQ_DISPLAY_CURVE_ST2084:
+            if (p->ContentColorSpace == VQ_COLOR_SPACE_REC_709) tonemap_kernel<VQ_DISPLAY_CURVE_ST2084, false, true, MULTI><<<grid, TM_THREADS, 0, s>>>(vi, vo, hdrScalar);
+            else                                                 tonemap_kernel<VQ_DISPLAY_CURVE_ST2084, false, false, MULTI><<<grid, TM_THREADS, 0, s>>>(vi, vo, hdrScalar);
+            break;
+        case VQ_DISPLAY_CURVE_LINEAR:
+            tonemap_kernel<VQ_DISPLAY_CURVE_LINEAR, false, false, MULTI><<<grid, TM_THREADS, 0, s>>>(vi, vo, hdrScalar);
+            break;
+        default:   // Tonemapper.hlsl:143-145: unknown curve paints yellow
+            tonemap_kernel<3, false, false, MULTI><<<grid, TM_THREADS, 0, s>>>(vi, vo, hdrScalar);
+            break;
     }
 }
 
@@ -79,25 +153,7 @@ extern "C" int vq_tonemap(VqContext* ctx, const VqTonemapperParams* p, VqImage i
     VQ_REQUIRE(vq_image_ok(in) && vq_image_ok(out), "bad image descriptor");
     VQ_REQUIRE(in.width == out.width && in.height == out.height, "tonemap: in/out size mismatch");
     const dim3 grid((in.width + TM_THREADS * TM_PX - 1) / (TM_THREADS * TM_PX), in.height);
-    const ImgV vi = make_view(in), vo = make_view(out);
-    cudaStream_t s = (cudaStream_t)stream;
-    const float hdrScalar = p->DisplayReferenceBrightnessLevel / 10000.0f;   // ST2084_MAX, HDR.hlsl:43
-    switch (p->OutputDisplayCurve) {
-        case VQ_DISPLAY_CURVE_SRGB:
-            if (p->ToggleGammaCorrection) tonemap_kernel<VQ_DISPLAY_CURVE_SRGB, true, false><<<grid, TM_THREADS, 0, s>>>(vi, vo, hdrScalar);
-            else                          tonemap_kernel<VQ_DISPLAY_CURVE_SRGB, false, false><<<grid, TM_THREADS, 0, s>>>(vi, vo, hdrScalar);
-            break;
-        case VQ_DISPLAY_CURVE_ST2084:
-            if (p->ContentColorSpace == VQ_COLOR_SPACE_REC_709) tonemap_kernel<VQ_DISPLAY_CURVE_ST2084, false, true><<<grid, TM_THREADS, 0, s>>>(vi, vo, hdrScalar);
-            else                                                 tonemap_kernel<VQ_DISPLAY_CURVE_ST2084, false, false><<<grid, TM_THREADS, 0, s>>>(vi, vo, hdrScalar);
-            break;
-        case VQ_DISPLAY_CURVE_LINEAR:
-            tonemap_kernel<VQ_DISPLAY_CURVE_LINEAR, false, false><<<grid, TM_THREADS, 0, s>>>(vi, vo, hdrScalar);
-            break;
-        default:   // Tonemapper.hlsl:143-145: unknown curve paints yellow
-            tonemap_kernel<3, false, false><<<grid, TM_THREADS, 0, s>>>(vi, vo, hdrScalar);
-            break;
-    }
+    tonemap_launch<false>(p, grid, make_view(in), make_view(out), (cudaStream_t)stream);
     return vq_check_launch("tonemap");
 }
 
@@ -267,9 +323,10 @@ __device__ __forceinline__ float3 load_zero_border(const ImgV& im, int x, int y)
 // =============================================================================================
 constexpr int ST_BX = 32, ST_BY = 8;   // 3x3 stencil kernels: 32x8 pixel blocks, rows shared through L1
 
-__global__ void __launch_bounds__(ST_BX * ST_BY) cas_kernel(ImgV in, ImgV out, float peak) {
-    const int x = blockIdx.x * ST_BX + threadIdx.x, y = blockIdx.y * ST_BY + threadIdx.y;
-    if (x >= out.w || y >= out.h) return;
+template <bool MULTI = false>
+__global__ void __launch_bounds__(ST_BX * ST_BY) cas_kernel(ImgV in, PostOut<MULTI> out, float peak) {
+    const int x = blockIdx.x * ST_BX + threadIdx.x, y = tile_row(out) * ST_BY + threadIdx.y;
+    if (x >= out.w || y >= out.h) { post_retire(out); return; }
     const float3 b = load_zero_border(in, x, y - 1);
     const float3 d = load_zero_border(in, x - 1, y);
     const float3 e = load_zero_border(in, x, y);
@@ -287,7 +344,8 @@ __global__ void __launch_bounds__(ST_BX * ST_BY) cas_kernel(ImgV in, ImgV out, f
     o.x = saturate((b.x * wG + d.x * wG + f.x * wG + h.x * wG + e.x) * rcpWeight);
     o.y = saturate((b.y * wG + d.y * wG + f.y * wG + h.y * wG + e.y) * rcpWeight);
     o.z = saturate((b.z * wG + d.z * wG + f.z * wG + h.z * wG + e.z) * rcpWeight);
-    st_stream(out.row(y) + x, make_float4(o.x, o.y, o.z, 1.0f));
+    store_px(out, x, y, make_float4(o.x, o.y, o.z, 1.0f));
+    post_retire(out);
 }
 
 extern "C" int vq_cas(VqContext* ctx, const uint32_t cas_const[8], VqImage in, VqImage out, void* stream) {
@@ -306,9 +364,10 @@ extern "C" int vq_cas(VqContext* ctx, const uint32_t cas_const[8], VqImage in, V
 // =============================================================================================
 // K9 RCAS — FSR1.0/ffx_fsr1.h:684-769, wrapper AMDFidelityFX.hlsl:335-376
 // =============================================================================================
-__global__ void __launch_bounds__(ST_BX * ST_BY) rcas_kernel(ImgV in, ImgV out, float sharp) {
-    const int x = blockIdx.x * ST_BX + threadIdx.x, y = blockIdx.y * ST_BY + threadIdx.y;
-    if (x >= out.w || y >= out.h) return;
+template <bool MULTI = false>
+__global__ void __launch_bounds__(ST_BX * ST_BY) rcas_kernel(ImgV in, PostOut<MULTI> out, float sharp) {
+    const int x = blockIdx.x * ST_BX + threadIdx.x, y = tile_row(out) * ST_BY + threadIdx.y;
+    if (x >= out.w || y >= out.h) { post_retire(out); return; }
     const float3 b = load_zero_border(in, x, y - 1);
     const float3 d = load_zero_border(in, x - 1, y);
     const float3 e = load_zero_border(in, x, y);
@@ -333,7 +392,8 @@ __global__ void __launch_bounds__(ST_BX * ST_BY) rcas_kernel(ImgV in, ImgV out, 
     o.x = (lobe * b.x + lobe * d.x + lobe * h.x + lobe * f.x + e.x) * rcpL;
     o.y = (lobe * b.y + lobe * d.y + lobe * h.y + lobe * f.y + e.y) * rcpL;
     o.z = (lobe * b.z + lobe * d.z + lobe * h.z + lobe * f.z + e.z) * rcpL;
-    st_stream(out.row(y) + x, make_float4(o.x, o.y, o.z, 1.0f));
+    store_px(out, x, y, make_float4(o.x, o.y, o.z, 1.0f));
+    post_retire(out);
 }
 
 extern "C" int vq_fsr_rcas(VqContext* ctx, const uint32_t rcas_const[4], VqImage in, VqImage out, void* stream) {
@@ -456,16 +516,17 @@ __device__ __forceinline__ float3 easu_filter(float ppx, float ppy, Tap tap) {
 }
 
 // Generic path (any scale): taps fetched straight from global memory through L1.
-template <int ADDR>
-__global__ void __launch_bounds__(ST_BX * ST_BY) easu_kernel(ImgV in, ImgV out, EasuCon con) {
-    const int x = blockIdx.x * ST_BX + threadIdx.x, y = blockIdx.y * ST_BY + threadIdx.y;
-    if (x >= out.w || y >= out.h) return;
+template <int ADDR, bool MULTI = false>
+__global__ void __launch_bounds__(ST_BX * ST_BY) easu_kernel(ImgV in, PostOut<MULTI> out, EasuCon con) {
+    const int x = blockIdx.x * ST_BX + threadIdx.x, y = tile_row(out) * ST_BY + threadIdx.y;
+    if (x >= out.w || y >= out.h) { post_retire(out); return; }
     float ppx = easu_pos(x, con.c0x, con.c0z), ppy = easu_pos(y, con.c0y, con.c0w);
     const float fpx = floorf(ppx), fpy = floorf(ppy);
     ppx -= fpx; ppy -= fpy;
     const int fx = (int)fpx, fy = (int)fpy;
     const float3 pix = easu_filter(ppx, ppy, [&](int dx, int dy) { return load_addr<ADDR>(in, fx + dx, fy + dy); });
-    st_stream(out.row(y) + x, make_float4(pix.x, pix.y, pix.z, 1.0f));
+    store_px(out, x, y, make_float4(pix.x, pix.y, pix.z, 1.0f));
+    post_retire(out);
 }
 
 // Upscaling path (input/output ratio <= 1, the FSR use case), two phases per CTA of 32x8 OUTPUT pixels:
@@ -511,11 +572,11 @@ __device__ __forceinline__ void easu_tap_v(float3& aC, float& aW, float vx, floa
     aW += w;
 }
 
-template <int ADDR>
-__global__ void __launch_bounds__(EU_BX * EU_BY, EU_BY <= 8 ? 4 : 2) easu_up_kernel(ImgV in, ImgV out, EasuCon con) {
+template <int ADDR, bool MULTI = false>
+__global__ void __launch_bounds__(EU_BX * EU_BY, EU_BY <= 8 ? 4 : 2) easu_up_kernel(ImgV in, PostOut<MULTI> out, EasuCon con) {
     __shared__ float4 tile[EU_TH][EU_TW];          // rgb + luma
     __shared__ float4 sets[4][EU_BY][EU_BX];       // S,T,U,V analyses of candidate texel (fy-fyFirst, fx-fxFirst); SoA: conflict-free
-    const int ox0 = blockIdx.x * EU_BX, oy0 = blockIdx.y * EU_BY;
+    const int ox0 = blockIdx.x * EU_BX, oy0 = tile_row(out) * EU_BY;
     const int fxFirst = (int)floorf(easu_pos(ox0, con.c0x, con.c0z));
     const int fyFirst = (int)floorf(easu_pos(oy0, con.c0y, con.c0w));
     const int tx0 = fxFirst - 1, ty0 = fyFirst - 1;
@@ -556,7 +617,7 @@ __global__ void __launch_bounds__(EU_BX * EU_BY, EU_BY <= 8 ? 4 : 2) easu_up_ker
     __syncthreads();
     // ---- phase 2: one output pixel per thread ----
     const int x = ox0 + threadIdx.x, y = oy0 + threadIdx.y;
-    if (x >= out.w || y >= out.h) return;
+    if (x >= out.w || y >= out.h) { post_retire(out); return; }
     float ppx = easu_pos(x, con.c0x, con.c0z), ppy = easu_pos(y, con.c0y, con.c0w);
     const float fpx = floorf(ppx), fpy = floorf(ppy);
     ppx -= fpx; ppy -= fpy;
@@ -607,7 +668,8 @@ __global__ void __launch_bounds__(EU_BX * EU_BY, EU_BY <= 8 ? 4 : 2) easu_up_ker
     easu_tap_v(aC, aW, vx2 + Ax, vy2 + Ay, lob, clp, t[2 * EU_TW + 1]);          // o (1,2)
     const float rw = rcp_fast(aW);
     const float3 pix = fmin3(max4, fmax3(min4, aC * rw));
-    st_stream(out.row(y) + x, make_float4(pix.x, pix.y, pix.z, 1.0f));
+    store_px(out, x, y, make_float4(pix.x, pix.y, pix.z, 1.0f));
+    post_retire(out);
 }
 
 // Exact 2x upscale (the FSR1 "performance" preset, BASELINE config 4): con0 = (0.5, 0.5, -0.25, -0.25), so the output pixels
@@ -660,11 +722,11 @@ __device__ __forceinline__ void easu2_tap(EasuAcc2& A, f2 vx, f2 vy, const EasuP
     A.w = A.w + w;
 }
 
-template <int ADDR>
-__global__ void __launch_bounds__(E2_BX * E2_BY, E2_MINB) easu_2x_kernel(ImgV in, ImgV out) {
+template <int ADDR, bool MULTI = false>
+__global__ void __launch_bounds__(E2_BX * E2_BY, E2_MINB) easu_2x_kernel(ImgV in, PostOut<MULTI> out) {
     __shared__ float4 tile[E2_TH][E2_TW];          // rgb + luma
     // 'f' texels of this CTA: k in [k0, k0+32), m in [m0, m0+8) with k0 = 32*bx - 1 (k = -1 owns output column 0)
-    const int k0 = (int)blockIdx.x * E2_BX - 1, m0 = (int)blockIdx.y * E2_BY - 1;
+    const int k0 = (int)blockIdx.x * E2_BX - 1, m0 = (int)tile_row(out) * E2_BY - 1;
     for (int i = threadIdx.y * E2_BX + threadIdx.x; i < E2_TH * E2_TW; i += E2_BX * E2_BY) {
         const int ly = i / E2_TW, lx = i - ly * E2_TW;
         const float3 v = load_addr<ADDR>(in, k0 - 1 + lx, m0 - 1 + ly);
@@ -673,7 +735,7 @@ __global__ void __launch_bounds__(E2_BX * E2_BY, E2_MINB) easu_2x_kernel(ImgV in
     __syncthreads();
     const int k = k0 + (int)threadIdx.x, m = m0 + (int)threadIdx.y;
     const int ox = 2 * k + 1, oy = 2 * m + 1;                        // top-left pixel of the quad
-    if (ox >= out.w || oy >= out.h) return;                          // (k, m) beyond the last owning texel
+    if (ox >= out.w || oy >= out.h) { post_retire(out); return; }    // (k, m) beyond the last owning texel
     const float4* t = &tile[threadIdx.y + 1][threadIdx.x + 1];      // 'f'
     float3 min4, max4;
     EasuSet S, T, U, V;
@@ -721,12 +783,13 @@ __global__ void __launch_bounds__(E2_BX * E2_BY, E2_MINB) easu_2x_kernel(ImgV in
         easu2_tap(A, vx2 + Ax, vy2 + Ay, P, t[2 * E2_TW + 1]);                                           // o (1,2)
         const f2 rw = rcp2(A.w);                                                           // ARcpF1 = rcp() in the HLSL
         const f2 cr = A.r * rw, cg = A.g * rw, cb = A.b * rw;
-        float4* dst = out.row(y);
-        if (ox >= 0) st_stream(dst + ox, make_float4(fminf(max4.x, fmaxf(min4.x, cr.v.x)), fminf(max4.y, fmaxf(min4.y, cg.v.x)),
-                                                     fminf(max4.z, fmaxf(min4.z, cb.v.x)), 1.0f));
-        if (ox + 1 < out.w) st_stream(dst + ox + 1, make_float4(fminf(max4.x, fmaxf(min4.x, cr.v.y)), fminf(max4.y, fmaxf(min4.y, cg.v.y)),
-                                                                fminf(max4.z, fmaxf(min4.z, cb.v.y)), 1.0f));
+        float4* dst = out_row(out, y);
+        if (ox >= 0) store_px(out, dst + ox, ox, y, make_float4(fminf(max4.x, fmaxf(min4.x, cr.v.x)), fminf(max4.y, fmaxf(min4.y, cg.v.x)),
+                                                      fminf(max4.z, fmaxf(min4.z, cb.v.x)), 1.0f));
+        if (ox + 1 < out.w) store_px(out, dst + ox + 1, ox + 1, y, make_float4(fminf(max4.x, fmaxf(min4.x, cr.v.y)), fminf(max4.y, fmaxf(min4.y, cg.v.y)),
+                                                                     fminf(max4.z, fmaxf(min4.z, cb.v.y)), 1.0f));
     }
+    post_retire(out);
 }
 
 extern "C" int vq_fsr_easu(VqContext* ctx, const uint32_t con[16], int address_mode, VqImage in, VqImage out, void* stream) {
@@ -762,6 +825,142 @@ extern "C" int vq_fsr_easu(VqContext* ctx, const uint32_t con[16], int address_m
         else                                 easu_kernel<VQ_ADDRESS_CLAMP><<<grid, dim3(ST_BX, ST_BY), 0, st>>>(make_view(in), make_view(out), c);
     }
     return vq_check_launch("fsr_easu");
+}
+
+// =============================================================================================
+// K6-K9 on a band of the output into several frames (vq_*_multi_signal): one rank's share of the post chain
+// =============================================================================================
+// The destination checks every multi-destination post call shares, before the device is touched: 1..8 destinations of exactly the
+// W x H output (`size_msg`, the single call's message, otherwise), none equal to `in` unless the pass may run in place
+// (`alias_msg` == nullptr: the tonemapper), then the row range and the signal as vq_multi_dest_check takes them. Fills `d`.
+static int post_dests_check(VqImage in, const VqImage* outs, int n_outs, int W, int H, const char* size_msg, const char* alias_msg,
+                            int row_begin, int row_end, const VqPeerSignal* sig, PostDests& d) {
+    VQ_REQUIRE(outs, "null destination list");
+    VQ_REQUIRE(n_outs >= 1 && n_outs <= 8, "1..8 destinations");
+    for (int k = 0; k < n_outs; ++k) {
+        VQ_REQUIRE(vq_image_ok(outs[k]), "bad image descriptor");
+        VQ_REQUIRE(outs[k].width == W && outs[k].height == H, size_msg);
+        VQ_REQUIRE(!alias_msg || outs[k].ptr != in.ptr, alias_msg);
+    }
+    memset(&d, 0, sizeof(d));
+    const int rc = vq_multi_dest_check(outs, n_outs, W, H, 0, row_begin, row_end, sig, d.sync); if (rc) return rc;
+    for (int k = 0; k < n_outs; ++k) d.o[k] = make_view(outs[k]);
+    d.n = n_outs; d.w = W; d.h = H; d.rowBegin = row_begin; d.rowEnd = row_end;
+    return VQ_OK;
+}
+
+static int floor_div(int a, int b) { return a >= 0 ? a / b : -((-a + b - 1) / b); }
+
+// Launch geometry of a MULTI kernel whose tile row `by` of `n_tiles` covers output rows [by * tile + lo, by * tile + hi]: the tile
+// rows that meet the range, [d.by0, d.by0 + count). Takes the rendezvous ticket when there is one.
+static unsigned post_tile_rows(VqContext* ctx, PostDests& d, int tile, int lo, int hi, int n_tiles) {
+    const int first = std::max(0, floor_div(d.rowBegin - hi + tile - 1, tile));
+    const int last = std::min(n_tiles - 1, floor_div(d.rowEnd - 1 - lo, tile));
+    d.by0 = first;
+    d.ticket = d.sync.n > 1 ? vq_ticket_pair(ctx) : nullptr;
+    return (unsigned)(last - first + 1);
+}
+
+extern "C" int vq_tonemap_multi_signal(VqContext* ctx, const VqTonemapperParams* p, VqImage in, const VqImage* outs, int n_outs,
+                                       int row_begin, int row_end, const VqPeerSignal* signal, void* stream) {
+    VQ_REQUIRE(p, "params is null");
+    VQ_REQUIRE(vq_image_ok(in), "bad image descriptor");
+    PostDests d;
+    int rc = post_dests_check(in, outs, n_outs, in.width, in.height, "tonemap: in/out size mismatch", nullptr, row_begin, row_end,
+                              signal, d); if (rc) return rc;
+    rc = vq_enter(ctx); if (rc) return rc;
+    VQ_MARK("TonemapperCS");
+    if (row_begin == row_end) return VQ_OK;
+    const unsigned gy = post_tile_rows(ctx, d, 1, 0, 0, in.height);
+    tonemap_launch<true>(p, dim3((in.width + TM_THREADS * TM_PX - 1) / (TM_THREADS * TM_PX), gy), make_view(in), d, (cudaStream_t)stream);
+    return vq_check_launch("tonemap_multi");
+}
+
+extern "C" int vq_cas_multi_signal(VqContext* ctx, const uint32_t cas_const[8], VqImage in, const VqImage* outs, int n_outs,
+                                   int row_begin, int row_end, const VqPeerSignal* signal, void* stream) {
+    VQ_REQUIRE(cas_const, "cas_const is null");
+    VQ_REQUIRE(vq_image_ok(in), "bad image descriptor");
+    PostDests d;
+    int rc = post_dests_check(in, outs, n_outs, in.width, in.height, "cas: sharpen-only path needs equal sizes (FFXCAS_NO_UPSCALING)",
+                              "cas: in-place is not supported", row_begin, row_end, signal, d); if (rc) return rc;
+    rc = vq_enter(ctx); if (rc) return rc;
+    VQ_MARK("FFX-CAS CS");
+    if (row_begin == row_end) return VQ_OK;
+    float peak; memcpy(&peak, &cas_const[4], 4);     // const1.x
+    const unsigned gy = post_tile_rows(ctx, d, ST_BY, 0, ST_BY - 1, (in.height + ST_BY - 1) / ST_BY);
+    cas_kernel<true><<<dim3((in.width + ST_BX - 1) / ST_BX, gy), dim3(ST_BX, ST_BY), 0, (cudaStream_t)stream>>>(make_view(in), d, peak);
+    return vq_check_launch("cas_multi");
+}
+
+extern "C" int vq_fsr_rcas_multi_signal(VqContext* ctx, const uint32_t rcas_const[4], VqImage in, const VqImage* outs, int n_outs,
+                                        int row_begin, int row_end, const VqPeerSignal* signal, void* stream) {
+    VQ_REQUIRE(rcas_const, "rcas_const is null");
+    VQ_REQUIRE(vq_image_ok(in), "bad image descriptor");
+    PostDests d;
+    int rc = post_dests_check(in, outs, n_outs, in.width, in.height, "rcas: in/out size mismatch", "rcas: in-place is not supported",
+                              row_begin, row_end, signal, d); if (rc) return rc;
+    rc = vq_enter(ctx); if (rc) return rc;
+    VQ_MARK("FSR-RCAS CS");
+    if (row_begin == row_end) return VQ_OK;
+    float sharp; memcpy(&sharp, &rcas_const[0], 4);
+    const unsigned gy = post_tile_rows(ctx, d, ST_BY, 0, ST_BY - 1, (in.height + ST_BY - 1) / ST_BY);
+    rcas_kernel<true><<<dim3((in.width + ST_BX - 1) / ST_BX, gy), dim3(ST_BX, ST_BY), 0, (cudaStream_t)stream>>>(make_view(in), d, sharp);
+    return vq_check_launch("fsr_rcas_multi");
+}
+
+extern "C" int vq_fsr_easu_multi_signal(VqContext* ctx, const uint32_t con[16], int address_mode, VqImage in, const VqImage* outs,
+                                        int n_outs, int row_begin, int row_end, const VqPeerSignal* signal, void* stream) {
+    VQ_REQUIRE(con, "easu_const is null");
+    VQ_REQUIRE(vq_image_ok(in), "bad image descriptor");
+    VQ_REQUIRE(address_mode == VQ_ADDRESS_WRAP || address_mode == VQ_ADDRESS_CLAMP, "easu: unknown address mode");
+    const int W = outs && n_outs >= 1 ? outs[0].width : 0, H = outs && n_outs >= 1 ? outs[0].height : 0;
+    PostDests d;
+    int rc = post_dests_check(in, outs, n_outs, W, H, "every destination must have the size of the first",
+                              "easu: in-place is not supported", row_begin, row_end, signal, d); if (rc) return rc;
+    EasuCon c; memcpy(&c, con, 16);
+    const float c0[4] = {c.c0x, c.c0y, c.c0z, c.c0w};
+    const vqeasu::Verdict v = vqeasu::check(c0, in.width, in.height, W, H);
+    VQ_REQUIRE(v != vqeasu::EASU_NONFINITE, "easu: con0 is not finite");
+    VQ_REQUIRE(v != vqeasu::EASU_TAPS_OUTSIDE, "easu: con0 puts taps outside [-w, 2w) x [-h, 2h) of the input (constants not built for these images?)");
+    VQ_REQUIRE(v != vqeasu::EASU_TILE_FOOTPRINT, "easu: con0 needs more than 32x8 input texels per 32x8 output tile");
+    rc = vq_enter(ctx); if (rc) return rc;
+    VQ_MARK("FSR-EASU CS");
+    if (row_begin == row_end) return VQ_OK;
+    cudaStream_t st = (cudaStream_t)stream;
+    const ImgV vi = make_view(in);
+    const bool wrap = address_mode == VQ_ADDRESS_WRAP;
+    const vqeasu::Path path = vqeasu::path(c0, in.width, in.height, W, H);
+    if (path == vqeasu::EASU_2X) {
+        // tile row `by` holds 'f' rows m0 = E2_BY * by - 1 .. m0 + E2_BY - 1, i.e. output rows 2 * m0 + 1 .. 2 * m0 + 2 * E2_BY
+        const unsigned gy = post_tile_rows(ctx, d, 2 * E2_BY, -1, 2 * E2_BY - 2, (in.height + 1 + E2_BY - 1) / E2_BY);
+        const dim3 grid((in.width + 1 + E2_BX - 1) / E2_BX, gy);
+        if (wrap) easu_2x_kernel<VQ_ADDRESS_WRAP, true><<<grid, dim3(E2_BX, E2_BY), 0, st>>>(vi, d);
+        else      easu_2x_kernel<VQ_ADDRESS_CLAMP, true><<<grid, dim3(E2_BX, E2_BY), 0, st>>>(vi, d);
+    } else if (path == vqeasu::EASU_UP) {
+        const unsigned gy = post_tile_rows(ctx, d, EU_BY, 0, EU_BY - 1, (H + EU_BY - 1) / EU_BY);
+        const dim3 grid((W + EU_BX - 1) / EU_BX, gy);
+        if (wrap) easu_up_kernel<VQ_ADDRESS_WRAP, true><<<grid, dim3(EU_BX, EU_BY), 0, st>>>(vi, d, c);
+        else      easu_up_kernel<VQ_ADDRESS_CLAMP, true><<<grid, dim3(EU_BX, EU_BY), 0, st>>>(vi, d, c);
+    } else {
+        const unsigned gy = post_tile_rows(ctx, d, ST_BY, 0, ST_BY - 1, (H + ST_BY - 1) / ST_BY);
+        const dim3 grid((W + ST_BX - 1) / ST_BX, gy);
+        if (wrap) easu_kernel<VQ_ADDRESS_WRAP, true><<<grid, dim3(ST_BX, ST_BY), 0, st>>>(vi, d, c);
+        else      easu_kernel<VQ_ADDRESS_CLAMP, true><<<grid, dim3(ST_BX, ST_BY), 0, st>>>(vi, d, c);
+    }
+    return vq_check_launch("fsr_easu_multi");
+}
+
+extern "C" int vq_fsr_easu_source_rows(const uint32_t con[16], int address_mode, int in_height, int out_height, int row_begin,
+                                       int row_end, int ranges[4]) {
+    VQ_REQUIRE(con && ranges, "null argument");
+    VQ_REQUIRE(address_mode == VQ_ADDRESS_WRAP || address_mode == VQ_ADDRESS_CLAMP, "easu: unknown address mode");
+    VQ_REQUIRE(in_height > 0 && out_height > 0, "heights must be positive");
+    VQ_REQUIRE(row_begin >= 0 && row_end <= out_height && row_begin <= row_end, "row range out of bounds");
+    EasuCon c; memcpy(&c, con, 16);
+    VQ_REQUIRE(isfinite(c.c0y) && isfinite(c.c0w), "easu: con0 is not finite");
+    VQ_REQUIRE(vqeasu::axis_ok(c.c0y, c.c0w, in_height, out_height),
+               "easu: con0 puts taps outside [-h, 2h) of the input (constants not built for these heights?)");
+    return vqeasu::source_rows(c.c0y, c.c0w, address_mode == VQ_ADDRESS_WRAP, in_height, row_begin, row_end, ranges);
 }
 
 // =============================================================================================

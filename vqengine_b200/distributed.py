@@ -6,7 +6,7 @@ finished tiles at the end (NCCL over NVLink on the GPU box; gloo in the CPU test
 GPU, torch.distributed for the plumbing. Nothing here computes pixels.
 
 Row spaces:
-  forward / post passes : image rows                      -> equal contiguous row blocks
+  forward / post passes : image rows                      -> equal contiguous row blocks (post chain halos: post_chain_rows)
   diffuse irradiance    : face*res + row                  -> equal contiguous row blocks
   specular prefilter    : flattened (mip, face, row)      -> contiguous blocks of equal COST
                           (a row of mip m has (res>>m) texels; mip 0 is roughness 0 = ~1 % of a full texel,
@@ -16,7 +16,7 @@ contiguous texel range of the packed buffer, so the gather needs no strided copi
 """
 from __future__ import annotations
 
-from typing import List, Sequence, Tuple
+from typing import Dict, List, Sequence, Tuple
 
 
 def equal_tiles(n_rows: int, world: int) -> List[Tuple[int, int]]:
@@ -31,6 +31,35 @@ def even_tiles(n_rows: int, world: int) -> List[Tuple[int, int]]:
     pairs = n_rows // 2
     cuts = [2 * (-(-pairs * r // world)) for r in range(world)] + [n_rows]
     return [(cuts[r], cuts[r + 1]) for r in range(world)]
+
+
+def post_chain_rows(in_height: int, out_height: int, band: Tuple[int, int], fsr_con=None, address_mode: int = 0,
+                    cas: bool = False) -> Dict[str, List[Tuple[int, int]]]:
+    """The [begin, end) rows each post pass must produce so that the chain's last pass can write rows `band` of the display frame
+    (DESIGN.md §6). Plumbing only: nothing is launched. The stages come in the order RenderPostProcess runs them, the last one
+    writing the display frame:
+      fsr_con given (FSR on): tonemap -> fsr_easu -> fsr_rcas; CAS is not run, its output is unused when FSR is on;
+      cas (FSR off, CAS on):  tonemap -> cas;
+      otherwise:              tonemap.
+    in_height is the HDR frame's height, out_height the display frame's (equal without FSR); address_mode is EASU's sampler
+    addressing (0 = WRAP, the engine's). RCAS and CAS read rows y-1 .. y+1 of their source: the band plus one row each side,
+    clipped to the image. EASU's source rows are vq_fsr_easu_source_rows's: one or, under WRAP at the top and bottom of the frame,
+    two ranges, so the tonemapper may run twice. An empty band gives empty lists."""
+    a, b = band
+    assert 0 <= a <= b <= out_height
+    if fsr_con is None:
+        assert in_height == out_height, "without FSR the display frame has the HDR frame's size"
+    if a == b:
+        stages = ("tonemap", "fsr_easu", "fsr_rcas") if fsr_con is not None else ("tonemap", "cas") if cas else ("tonemap",)
+        return {s: [] for s in stages}
+    halo = (max(a - 1, 0), min(b + 1, out_height))
+    if fsr_con is not None:
+        from . import fsr_easu_source_rows
+        return {"tonemap": fsr_easu_source_rows(fsr_con, in_height, out_height, *halo, address_mode=address_mode),
+                "fsr_easu": [halo], "fsr_rcas": [(a, b)]}
+    if cas:
+        return {"tonemap": [halo], "cas": [(a, b)]}
+    return {"tonemap": [(a, b)]}
 
 
 def weighted_tiles(costs: Sequence[float], world: int) -> List[Tuple[int, int]]:
