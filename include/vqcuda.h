@@ -490,7 +490,15 @@ VQ_API int vq_hdr_decode(VqContext* ctx, const void* dev_file, uint64_t size, co
                          const uint64_t* dev_channel_offsets, VqImage out, float* dev_max_luminance, void* stream);
 /* Blocking: host file image -> device fp32 image (parse + upload + decode). */
 VQ_API int vq_hdr_load_host(VqContext* ctx, const void* host_file, uint64_t size, VqImage out, float* max_luminance);
-/* DEVICE. RGBA32F -> RGBE texels (4 bytes each, tightly packed rows), stbiw__linear_to_rgbe. Inputs are radiance (>= 0). */
+/* DEVICE. RGBA32F -> RGBE texels (4 bytes each, tightly packed rows), stbiw__linear_to_rgbe, for every float input:
+ *   maxcomp = max(r, max(g, b)) with max(a, b) = a > b ? a : b, stb's nesting: a NaN in r or g is ignored
+ *   (the comparison is false, so the other operand is taken), a NaN in b is not;
+ *   maxcomp < 1e-32 (negative values, -0 and -Inf included) -> (0, 0, 0, 0);
+ *   otherwise e = the frexp exponent of maxcomp (0 for +Inf and NaN), exponent byte = (e + 128) & 0xff, so maxcomp >= 2^127
+ *   wraps it to 0 and the texel decodes as black (stb writes the same bytes and reads them back the same way);
+ *   channel byte = the low byte of c * 2^(8 - e) truncated toward zero to int32 (a negative channel wraps, a NaN product
+ *   gives 0: maxcomp = +Inf or NaN writes (0, 0, 0, 128); maxcomp = -Inf is below the cut-off and writes
+ *   (0, 0, 0, 0)). */
 VQ_API int vq_hdr_encode_rgbe(VqContext* ctx, VqImage in, void* dev_rgbe, void* stream);
 /* HOST. RGBE texels -> the .hdr file image (text header + per-scanline run lists). file == NULL: size query. */
 VQ_API int vq_hdr_pack_file(const void* host_rgbe, int width, int height, void* file, uint64_t capacity, uint64_t* size);
@@ -503,6 +511,10 @@ VQ_API int vq_hdr_save_host(VqContext* ctx, VqImage in, void* host_file, uint64_
  * v0.96. out.width <= in.width and out.height <= in.height (otherwise VQ_ERR_UNSUPPORTED). The intermediate image and the gather
  * tables live in the context (grow-only; tables are rebuilt when the size pair changes): serialise calls per context. */
 VQ_API int vq_image_resize(VqContext* ctx, VqImage in, VqImage out, void* stream);
+/* Non-finite inputs: stb adds a coefficient only where it is nonzero. The gather tables start and end every output's taps at
+ * a nonzero weight, so +-Inf and NaN reach the same outputs as in stb, with one exception: at ratios where a Mitchell weight
+ * rounds to exactly 0 between two taps of an output (|x| = 8/7; 7:5, for example), the kernels add 0 * Inf = NaN where stb
+ * adds nothing. Finite inputs are bit-identical either way. */
 /* HOST. The per-axis gather table vq_image_resize builds (first tap, tap count, normalised weights per output sample):
  * out[i] = sum_{t<count[i]} weights[i*capacity_taps + t] * in[clamp(start[i]+t, 0, in_size-1)], taps in increasing order.
  * start == NULL: only *max_taps is written. */
@@ -515,7 +527,9 @@ VQ_API int vq_resize_axis_table(int in_size, int out_size, int* start, int* coun
  *     skyCam.Proj, Scene.cpp:573-584; row-vector convention), computed by the caller. The pass writes {rgb, 1} to
  *     rows [row_begin,row_end) of scene_color where no surface was shaded: pixels whose normal_mask texel has
  *     xyz == 0 (the G-buffer normal plane; the engine gets the same effect from the depth test), or every pixel when
- *     normal_mask is NULL.
+ *     normal_mask is NULL. A ray that keeps no direction (its w rounds to 0, or |ray / w|^2 overflows fp32) is drawn black.
+ *     Signed zeros follow atan2: the centre pixel of an axis-aligned camera looking along +-Y whose ray has x = -0 maps to
+ *     u = 0 or 1 (the -X seam), not to u = 0.5.
  *   ApplyReflections: replaces CSMain (ApplyReflections.hlsl:31-57): scene.rgb += reflection.rgb, alpha kept;
  *     with a bounding_volumes layer (COMPOSITE_BOUNDING_VOLUMES) the sum is blended under it. In place.
  * ------------------------------------------------------------------------------------------ */
@@ -543,7 +557,11 @@ VQ_API int vq_apply_reflections(VqContext* ctx, VqImage scene_color, VqImage ref
  *     level above; `levels` receives n_levels (<= vq_depth_pyramid_level_count = 1 + floor(log2(max(w,h))), at most 13)
  *     tightly packed levels, vq_depth_pyramid_texel_count() floats in total. The padded-domain levels ping-pong through scratch
  *     owned by the context (like vq_image_resize): calls on ONE context must be issued on one stream at a time.
- *   Parity: tests/test_shadow_gpu.py (15 tests against the oracle, itself pinned to the reference's shader text).
+ *     The minimum ignores NaN unless all four texels are NaN. Where the smallest value of a 2x2 block is a zero and zeros of
+ *     both signs reach it (a +0 and a -0 depth, or a -0 next to the zero padding), the sign of the result is not specified,
+ *     as D3D's min leaves it; every other result, denormals and infinities included, is exact.
+ *   Parity: tests/test_shadow_gpu.py (15 tests against the oracle, itself pinned to the reference's shader text) and
+ *     tests/test_frame_domain_gpu.py (every size edge, special depths, every n_levels, unaligned sources).
  * ------------------------------------------------------------------------------------------ */
 typedef struct VqShadowMaps {
     const void* point_cubes;     int32_t point_res;

@@ -139,17 +139,29 @@ float CalculateMaxLuminance(const float* rgba, int width, int height) {
     return MaxLuminance;
 }
 
-// stbiw__linear_to_rgbe (stb_image_write.h). The (unsigned char) casts of negative products are undefined in C;
-// inputs here are radiance (>= 0).
+// stbiw__linear_to_rgbe (stb_image_write.h). maxcomp is stbiw__max(r, stbiw__max(g, b)) with stbiw__max(a, b) = a > b ? a : b,
+// so a NaN in r or g is ignored (the comparison is false and the other operand is taken) and a NaN in b is not. C leaves
+// the (unsigned char) cast of a negative, NaN or huge product undefined; the bytes are pinned to the rule vqcuda.h states
+// for vq_hdr_encode_rgbe: the low byte of the product truncated to int32 (NaN -> 0, saturated at the int32 range). frexp
+// gives exponent 0 for +Inf and NaN (-Inf is below the cut-off); an exponent of 128 (maxcomp >= 2^127) wraps the byte to 0.
+static uint8_t TruncByte(float x) {
+    if (std::isnan(x)) return 0;
+    if (x >= 2147483648.0f) return 0xff;
+    if (x <= -2147483648.0f) return 0;
+    return (uint8_t)((int32_t)x & 0xff);
+}
 void LinearToRgbe(uint8_t rgbe[4], const float linear[3]) {
-    const float maxcomp = std::fmax(linear[0], std::fmax(linear[1], linear[2]));
+    const float gb = linear[1] > linear[2] ? linear[1] : linear[2];
+    const float maxcomp = linear[0] > gb ? linear[0] : gb;
     if (maxcomp < 1e-32f) { rgbe[0] = rgbe[1] = rgbe[2] = rgbe[3] = 0; return; }
-    int exponent;
-    const float normalize = (float)std::frexp(maxcomp, &exponent) * 256.0f / maxcomp;
-    rgbe[0] = (uint8_t)(linear[0] * normalize);
-    rgbe[1] = (uint8_t)(linear[1] * normalize);
-    rgbe[2] = (uint8_t)(linear[2] * normalize);
-    rgbe[3] = (uint8_t)(exponent + 128);
+    int exponent = 0;
+    const float mant = (float)std::frexp(maxcomp, &exponent);
+    if (!std::isfinite(maxcomp)) exponent = 0;
+    const float normalize = mant * 256.0f / maxcomp;
+    rgbe[0] = TruncByte(linear[0] * normalize);
+    rgbe[1] = TruncByte(linear[1] * normalize);
+    rgbe[2] = TruncByte(linear[2] * normalize);
+    rgbe[3] = (uint8_t)((exponent + 128) & 0xff);
 }
 
 // stbi_write_hdr_core with comp = 4 (Image.cpp:212): header + one RLE (or flat) scanline per row
