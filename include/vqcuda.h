@@ -341,6 +341,33 @@ VQ_API int vq_fsr_rcas_multi_signal(VqContext* ctx, const uint32_t rcas_const[4]
                                     int row_begin, int row_end, const VqPeerSignal* signal, void* stream);
 
 /* ------------------------------------------------------------------------------------------
+ * K6-K9 fused: RenderPostProcess in one launch (SceneRendering.cpp:2640-2781), from scene colour to display frame with no
+ *     intermediate image in device memory. The tonemapper, then FSR1 EASU + RCAS when easu_const != NULL (rcas_const required),
+ *     else CAS when cas_const != NULL, else the tonemapper alone (vq_tonemap's kernel). A NULL constant block turns its pass off;
+ *     with FSR on, cas_const is ignored (the engine does not read CAS's output then). address_mode is EASU's (vq_fsr_easu).
+ *     The display frame equals, bit for bit, vq_tonemap -> vq_fsr_easu -> vq_fsr_rcas, vq_tonemap -> vq_cas, or vq_tonemap.
+ *     Output alpha: 1 with EASU/RCAS or CAS, the input's alpha otherwise. One launch per call, no context scratch: calls on
+ *     several streams of one context are fine. The display is the size of scene_color without FSR, any size con0 was built for
+ *     with it.
+ *     Refused with VQ_ERR_INVALID_ARG before the device is touched (also with a NULL context): null params, bad descriptors,
+ *     the size rules of vq_tonemap / vq_cas, scene_color equal to the display with EASU/RCAS or CAS, an unknown address mode,
+ *     EASU's con0 checks (vq_fsr_easu) with the footprint bound of this kernel's tiles (on the upscaling path, a 30 x 14 display
+ *     tile and its 1-pixel ring may need at most 32 x 16 input texels), con0 on EASU's downscaling path (neither the exact 2x
+ *     nor 0 < con0.x, con0.y <= 1: run the three calls for those), and easu_const without rcas_const or the reverse.
+ *   vq_post_process_multi_signal: one rank's band of the display frame into several frames, as the K6-K9 multi-destination
+ *     calls above store theirs. Rows [row_begin,row_end) are rows of the DISPLAY frame; scene_color is the whole frame (the
+ *     halo rows are read, not planned); each of the n_outs (1..8) destinations has the size of outs[0], the display size.
+ *     Also refused: their destination, row and signal checks.
+ * ------------------------------------------------------------------------------------------ */
+VQ_API int vq_post_process(VqContext* ctx, const VqTonemapperParams* tonemapper, const uint32_t cas_const[8],
+                           const uint32_t easu_const[16], int address_mode, const uint32_t rcas_const[4],
+                           VqImage scene_color, VqImage display, void* stream);
+VQ_API int vq_post_process_multi_signal(VqContext* ctx, const VqTonemapperParams* tonemapper, const uint32_t cas_const[8],
+                                        const uint32_t easu_const[16], int address_mode, const uint32_t rcas_const[4],
+                                        VqImage scene_color, const VqImage* outs, int n_outs, int row_begin, int row_end,
+                                        const VqPeerSignal* signal, void* stream);
+
+/* ------------------------------------------------------------------------------------------
  * K10 FidelityFX SPD: the whole mip chain in one launch.  Replaces SPD_CSMain
  *     (AMDFidelityFX.hlsl:525-545) -> SpdDownsample (SPD/ffx_spd.h:811-835), reduction =
  *     (v0+v1+v2+v3)*0.25 (AMDFidelityFX.hlsl:463-466). `mips` are the destination levels

@@ -37,7 +37,7 @@ ABI_SYMBOLS = [
     "vq_forward_lighting_from_materials", "vq_forward_lighting_shadowed_from_materials",
     "vq_forward_lighting_shadowed_multi_signal", "vq_forward_lighting_from_materials_multi_signal",
     "vq_tonemap_multi_signal", "vq_cas_multi_signal", "vq_fsr_easu_multi_signal", "vq_fsr_rcas_multi_signal",
-    "vq_fsr_easu_source_rows",
+    "vq_fsr_easu_source_rows", "vq_post_process", "vq_post_process_multi_signal",
 ]
 
 
@@ -88,6 +88,9 @@ def _load() -> C.CDLL:
     lib.vq_cas_multi_signal.argtypes = [vp, P(u32), Image, P(Image), C.c_int, C.c_int, C.c_int, P(PeerSignal), vp]
     lib.vq_fsr_easu_multi_signal.argtypes = [vp, P(u32), C.c_int, Image, P(Image), C.c_int, C.c_int, C.c_int, P(PeerSignal), vp]
     lib.vq_fsr_rcas_multi_signal.argtypes = [vp, P(u32), Image, P(Image), C.c_int, C.c_int, C.c_int, P(PeerSignal), vp]
+    lib.vq_post_process.argtypes = [vp, P(TonemapperParams), P(u32), P(u32), C.c_int, P(u32), Image, Image, vp]
+    lib.vq_post_process_multi_signal.argtypes = [vp, P(TonemapperParams), P(u32), P(u32), C.c_int, P(u32), Image, P(Image), C.c_int,
+                                                 C.c_int, C.c_int, P(PeerSignal), vp]
     lib.vq_fsr_easu_source_rows.argtypes = [P(u32), C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, P(C.c_int)]
     lib.vq_fsr_easu_con.argtypes = [P(u32), f32, f32, f32, f32, f32, f32]
     lib.vq_fsr_easu_con.restype = None
@@ -575,6 +578,16 @@ class Context:
 
     def fsr_rcas_multi(self, con, src, out_images, row_begin=0, row_end=None, stream=None, signal=None):
         self._post_multi(lib.vq_fsr_rcas_multi_signal, (con,), src, out_images, row_begin, row_end, stream, signal)
+
+    # RenderPostProcess in one launch: tonemapper, then EASU + RCAS (easu and rcas given), else CAS (cas given), else nothing more
+    def post_process(self, tm: TonemapperParams, src, dst, cas=None, easu=None, rcas=None, address_mode=VQ_ADDRESS_WRAP, stream=None):
+        _check(lib.vq_post_process(self._h, C.byref(tm), cas, easu, address_mode, rcas, image_of(src), image_of(dst), _stream_ptr(stream)))
+
+    def post_process_multi(self, tm: TonemapperParams, src, out_images, row_begin=0, row_end=None, cas=None, easu=None, rcas=None,
+                           address_mode=VQ_ADDRESS_WRAP, stream=None, signal=None):
+        """post_process on display rows [row_begin, row_end) into every destination (Image descriptors, the local frame first)"""
+        self._post_multi(lib.vq_post_process_multi_signal, (C.byref(tm), cas, easu, address_mode, rcas), src, out_images, row_begin,
+                         row_end, stream, signal)
 
     def spd_downsample(self, constants: SpdConstants, src, mips, stream=None):
         arr = (Image * len(mips))(*[image_of(m) for m in mips])

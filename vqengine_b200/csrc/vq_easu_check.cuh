@@ -10,7 +10,8 @@
 //     the image with one add or subtract, which is right only in that range (images under 3 texels use the general % and
 //     any tap in the range);
 //   * the up path (0 < scale <= 1 on both axes, not the exact 2x) would need more candidate 'f' texels per 32 x 8 output tile
-//     than its shared-memory arrays hold (ncx > 32 or ncy > 8).
+//     than its shared-memory arrays hold (ncx > 32 or ncy > 8). The fused post kernel (vq_post_process) runs the up path on
+//     its 30 x 14 display tiles widened by RCAS's 1-pixel ring and holds 32 x 16 candidates: check(..., FUSED_UP_TILE).
 // Every con0 that FsrEasuCon builds for the image (viewport <= input size) passes: its taps lie in [-2, width + 1].
 #pragma once
 #include <math.h>
@@ -20,6 +21,12 @@ namespace vqeasu {
 enum Path { EASU_GENERIC = 0, EASU_UP = 1, EASU_2X = 2 };
 enum Verdict { EASU_OK = 0, EASU_NONFINITE = 1, EASU_TAPS_OUTSIDE = 2, EASU_TILE_FOOTPRINT = 3 };
 constexpr int UP_TILE_X = 32, UP_TILE_Y = 8;   // easu_up_kernel's output tile and its candidate-texel capacity
+
+// The up path's output tiles along x and y, the ring of extra outputs EASU computes around each (clipped to the output), and
+// the candidate 'f' texels the kernel can hold per widened tile
+struct UpTile { int x, y, ring, cap_x, cap_y; };
+constexpr UpTile EASU_UP_TILE = {UP_TILE_X, UP_TILE_Y, 0, UP_TILE_X, UP_TILE_Y};   // easu_up_kernel
+constexpr UpTile FUSED_UP_TILE = {30, 14, 1, 32, 16};                              // post_fsr_up_kernel (vq_post.cu)
 
 // the kernels' easu_pos (__fmul_rn then __fadd_rn); the product goes through a volatile so that no host compiler fuses it
 inline float pos(int o, float scale, float bias) {
@@ -33,12 +40,14 @@ inline Path path(const float c[4], int in_w, int in_h, int out_w, int out_h) {
     return EASU_GENERIC;
 }
 
-// largest number of candidate 'f' texels over the up path's tiles of `tile` outputs along one axis
-inline int max_candidates(float scale, float bias, int n_out, int tile) {
+// largest number of candidate 'f' texels over the up path's tiles of `tile` outputs along one axis, each widened by `ring`
+// outputs on both sides and clipped to [0, n_out)
+inline int max_candidates(float scale, float bias, int n_out, int tile, int ring = 0) {
     int worst = 0;
     for (int o0 = 0; o0 < n_out; o0 += tile) {
-        const int ol = o0 + tile - 1 < n_out - 1 ? o0 + tile - 1 : n_out - 1;
-        const int n = (int)floorf(pos(ol, scale, bias)) - (int)floorf(pos(o0, scale, bias)) + 1;
+        const int of = o0 - ring > 0 ? o0 - ring : 0;
+        const int ol = o0 + tile - 1 + ring < n_out - 1 ? o0 + tile - 1 + ring : n_out - 1;
+        const int n = (int)floorf(pos(ol, scale, bias)) - (int)floorf(pos(of, scale, bias)) + 1;
         worst = n > worst ? n : worst;
     }
     return worst;
@@ -54,18 +63,20 @@ inline bool axis_ok(float scale, float bias, int n_in, int n_out) {
     return lo >= -size && hi < 2.0 * size;
 }
 
-// c = con0 (scale x, scale y, bias x, bias y); ncx / ncy (may be null) receive the up path's largest tile footprint, 0 elsewhere
-inline Verdict check(const float c[4], int in_w, int in_h, int out_w, int out_h, int* ncx = nullptr, int* ncy = nullptr) {
+// c = con0 (scale x, scale y, bias x, bias y); ncx / ncy (may be null) receive the up path's largest tile footprint, 0 elsewhere;
+// `tile` is the up path's tiling (easu_up_kernel's unless given)
+inline Verdict check(const float c[4], int in_w, int in_h, int out_w, int out_h, int* ncx = nullptr, int* ncy = nullptr,
+                     const UpTile& tile = EASU_UP_TILE) {
     if (ncx) *ncx = 0;
     if (ncy) *ncy = 0;
     for (int i = 0; i < 4; ++i)
         if (!isfinite(c[i])) return EASU_NONFINITE;
     if (!axis_ok(c[0], c[2], in_w, out_w) || !axis_ok(c[1], c[3], in_h, out_h)) return EASU_TAPS_OUTSIDE;
     if (path(c, in_w, in_h, out_w, out_h) != EASU_UP) return EASU_OK;
-    const int nx = max_candidates(c[0], c[2], out_w, UP_TILE_X), ny = max_candidates(c[1], c[3], out_h, UP_TILE_Y);
+    const int nx = max_candidates(c[0], c[2], out_w, tile.x, tile.ring), ny = max_candidates(c[1], c[3], out_h, tile.y, tile.ring);
     if (ncx) *ncx = nx;
     if (ncy) *ncy = ny;
-    return nx <= UP_TILE_X && ny <= UP_TILE_Y ? EASU_OK : EASU_TILE_FOOTPRINT;
+    return nx <= tile.cap_x && ny <= tile.cap_y ? EASU_OK : EASU_TILE_FOOTPRINT;
 }
 
 // The input rows the kernels read for output rows [rb, re) of an axis that axis_ok accepts: the taps f-1 .. f+2 of every

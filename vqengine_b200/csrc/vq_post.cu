@@ -1,5 +1,5 @@
 // vq_post.cu — post chain kernels for sm_90a: Tonemapper (K6), separable Gaussian blur (K5),
-// FidelityFX CAS (K7), FSR1 EASU (K8) / RCAS (K9), SPD (K10).
+// FidelityFX CAS (K7), FSR1 EASU (K8) / RCAS (K9), SPD (K10), and K6-K9 fused into one launch (vq_post_process).
 //
 // All are streaming kernels over RGBA32F rows: float4 (LDG.128/STG.128) coalesced accesses, inputs
 // that are read once bypass L1 allocation, stencil inputs are staged in shared memory (blur) or
@@ -323,15 +323,8 @@ __device__ __forceinline__ float3 load_zero_border(const ImgV& im, int x, int y)
 // =============================================================================================
 constexpr int ST_BX = 32, ST_BY = 8;   // 3x3 stencil kernels: 32x8 pixel blocks, rows shared through L1
 
-template <bool MULTI = false>
-__global__ void __launch_bounds__(ST_BX * ST_BY) cas_kernel(ImgV in, PostOut<MULTI> out, float peak) {
-    const int x = blockIdx.x * ST_BX + threadIdx.x, y = tile_row(out) * ST_BY + threadIdx.y;
-    if (x >= out.w || y >= out.h) { post_retire(out); return; }
-    const float3 b = load_zero_border(in, x, y - 1);
-    const float3 d = load_zero_border(in, x - 1, y);
-    const float3 e = load_zero_border(in, x, y);
-    const float3 f = load_zero_border(in, x + 1, y);
-    const float3 h = load_zero_border(in, x, y + 1);
+// the CAS arithmetic of pixel e from its cross b (above), d (left), f (right), h (below); cas_kernel and post_cas_kernel
+__device__ __forceinline__ float3 cas_px(float3 b, float3 d, float3 e, float3 f, float3 h, float peak) {
     // only the green channel's weight survives without CAS_SLOW (ffx_cas.h:511-519)
     const float mnG = min3f(min3f(d.y, e.y, f.y), b.y, h.y);
     const float mxG = max3f(max3f(d.y, e.y, f.y), b.y, h.y);
@@ -344,6 +337,15 @@ __global__ void __launch_bounds__(ST_BX * ST_BY) cas_kernel(ImgV in, PostOut<MUL
     o.x = saturate((b.x * wG + d.x * wG + f.x * wG + h.x * wG + e.x) * rcpWeight);
     o.y = saturate((b.y * wG + d.y * wG + f.y * wG + h.y * wG + e.y) * rcpWeight);
     o.z = saturate((b.z * wG + d.z * wG + f.z * wG + h.z * wG + e.z) * rcpWeight);
+    return o;
+}
+
+template <bool MULTI = false>
+__global__ void __launch_bounds__(ST_BX * ST_BY) cas_kernel(ImgV in, PostOut<MULTI> out, float peak) {
+    const int x = blockIdx.x * ST_BX + threadIdx.x, y = tile_row(out) * ST_BY + threadIdx.y;
+    if (x >= out.w || y >= out.h) { post_retire(out); return; }
+    const float3 o = cas_px(load_zero_border(in, x, y - 1), load_zero_border(in, x - 1, y), load_zero_border(in, x, y),
+                            load_zero_border(in, x + 1, y), load_zero_border(in, x, y + 1), peak);
     store_px(out, x, y, make_float4(o.x, o.y, o.z, 1.0f));
     post_retire(out);
 }
@@ -364,15 +366,8 @@ extern "C" int vq_cas(VqContext* ctx, const uint32_t cas_const[8], VqImage in, V
 // =============================================================================================
 // K9 RCAS — FSR1.0/ffx_fsr1.h:684-769, wrapper AMDFidelityFX.hlsl:335-376
 // =============================================================================================
-template <bool MULTI = false>
-__global__ void __launch_bounds__(ST_BX * ST_BY) rcas_kernel(ImgV in, PostOut<MULTI> out, float sharp) {
-    const int x = blockIdx.x * ST_BX + threadIdx.x, y = tile_row(out) * ST_BY + threadIdx.y;
-    if (x >= out.w || y >= out.h) { post_retire(out); return; }
-    const float3 b = load_zero_border(in, x, y - 1);
-    const float3 d = load_zero_border(in, x - 1, y);
-    const float3 e = load_zero_border(in, x, y);
-    const float3 f = load_zero_border(in, x + 1, y);
-    const float3 h = load_zero_border(in, x, y + 1);
+// the RCAS arithmetic of pixel e from its cross b (above), d (left), f (right), h (below); rcas_kernel and the fused FSR kernels
+__device__ __forceinline__ float3 rcas_px(float3 b, float3 d, float3 e, float3 f, float3 h, float sharp) {
     const float3 mn4 = f3(fminf(min3f(b.x, d.x, f.x), h.x), fminf(min3f(b.y, d.y, f.y), h.y), fminf(min3f(b.z, d.z, f.z), h.z));
     const float3 mx4 = f3(fmaxf(max3f(b.x, d.x, f.x), h.x), fmaxf(max3f(b.y, d.y, f.y), h.y), fmaxf(max3f(b.z, d.z, f.z), h.z));
     // limiters use the full-precision rcp of the HLSL (ffx_fsr1.h:749-755), i.e. the hardware reciprocal (1 ulp)
@@ -392,6 +387,15 @@ __global__ void __launch_bounds__(ST_BX * ST_BY) rcas_kernel(ImgV in, PostOut<MU
     o.x = (lobe * b.x + lobe * d.x + lobe * h.x + lobe * f.x + e.x) * rcpL;
     o.y = (lobe * b.y + lobe * d.y + lobe * h.y + lobe * f.y + e.y) * rcpL;
     o.z = (lobe * b.z + lobe * d.z + lobe * h.z + lobe * f.z + e.z) * rcpL;
+    return o;
+}
+
+template <bool MULTI = false>
+__global__ void __launch_bounds__(ST_BX * ST_BY) rcas_kernel(ImgV in, PostOut<MULTI> out, float sharp) {
+    const int x = blockIdx.x * ST_BX + threadIdx.x, y = tile_row(out) * ST_BY + threadIdx.y;
+    if (x >= out.w || y >= out.h) { post_retire(out); return; }
+    const float3 o = rcas_px(load_zero_border(in, x, y - 1), load_zero_border(in, x - 1, y), load_zero_border(in, x, y),
+                             load_zero_border(in, x + 1, y), load_zero_border(in, x, y + 1), sharp);
     store_px(out, x, y, make_float4(o.x, o.y, o.z, 1.0f));
     post_retire(out);
 }
@@ -572,6 +576,72 @@ __device__ __forceinline__ void easu_tap_v(float3& aC, float& aW, float vx, floa
     aW += w;
 }
 
+// Phase 1 for candidate 'f' = t[0] of a staged footprint with row stride TW: its S, T, U, V analyses as {dirX, dirY, lenX, lenY}
+template <int TW>
+__device__ __forceinline__ void easu_up_sets(const float4* t, float4& aS, float4& aT, float4& aU, float4& aV) {
+    const float bL = t[-TW].w, cL = t[-TW + 1].w;
+    const float eL = t[-1].w, fL = t[0].w, gL = t[1].w, hL = t[2].w;
+    const float iL = t[TW - 1].w, jL = t[TW].w, kL = t[TW + 1].w, lL = t[TW + 2].w;
+    const float nL = t[2 * TW].w, oL = t[2 * TW + 1].w;
+    const EasuSet sS = easu_set_shared(bL, eL, fL, gL, jL), sT = easu_set_shared(cL, fL, gL, hL, kL);
+    const EasuSet sU = easu_set_shared(fL, iL, jL, kL, nL), sV = easu_set_shared(gL, jL, kL, lL, oL);
+    aS = make_float4(sS.dirX, sS.dirY, sS.lenX, sS.lenY);
+    aT = make_float4(sT.dirX, sT.dirY, sT.lenX, sT.lenY);
+    aU = make_float4(sU.dirX, sU.dirY, sU.lenX, sU.lenY);
+    aV = make_float4(sV.dirX, sV.dirY, sV.lenX, sV.lenY);
+}
+
+// Phase 2: the output pixel at fractional position (ppx, ppy) from 'f' = t[0] (row stride TW) and f's four analyses
+template <int TW>
+__device__ __forceinline__ float3 easu_up_px(const float4* t, const float4& aS, const float4& aT, const float4& aU, const float4& aV,
+                                             float ppx, float ppy) {
+    float2 dir = make_float2(0.0f, 0.0f);
+    float len = 0.0f;
+    easu_set_blend(dir, len, (1.0f - ppx) * (1.0f - ppy), aS);
+    easu_set_blend(dir, len, ppx * (1.0f - ppy), aT);
+    easu_set_blend(dir, len, (1.0f - ppx) * ppy, aU);
+    easu_set_blend(dir, len, ppx * ppy, aV);
+    float dirR = dir.x * dir.x + dir.y * dir.y;
+    const bool zro = dirR < (1.0f / 32768.0f);
+    dirR = APrxLoRsqF1(dirR);
+    dirR = zro ? 1.0f : dirR;
+    dir.x = zro ? 1.0f : dir.x;
+    dir.x *= dirR; dir.y *= dirR;
+    len = len * 0.5f;
+    len *= len;
+    const float stretch = (dir.x * dir.x + dir.y * dir.y) * APrxLoRcpF1(fmaxf(fabsf(dir.x), fabsf(dir.y)));
+    const float lenx = fmaf(stretch - 1.0f, len, 1.0f), leny = fmaf(-0.5f, len, 1.0f);
+    const float lob = fmaf((1.0f / 4.0f - 0.04f) - 0.5f, len, 0.5f);
+    const float clp = APrxLoRcpF1(lob);
+    // rotated + scaled offset of tap (i,j):  vx = ((i-ppx)*dir.x + (j-ppy)*dir.y)*lenx,  vy = (-(i-ppx)*dir.y + (j-ppy)*dir.x)*leny
+    const float Ax = dir.x * lenx, Bx = dir.y * lenx;        // d vx / d i , d vx / d j
+    const float Ay = -dir.y * leny, By = dir.x * leny;       // d vy / d i , d vy / d j
+    const float vx00 = -(ppx * Ax + ppy * Bx), vy00 = -(ppx * Ay + ppy * By);
+    const float4 tf = t[0], tg = t[1], tj = t[TW], tk = t[TW + 1];
+    const float3 min4 = fmin3(fmin3(xyz(tf), fmin3(xyz(tg), xyz(tj))), xyz(tk));
+    const float3 max4 = fmax3(fmax3(xyz(tf), fmax3(xyz(tg), xyz(tj))), xyz(tk));
+    float3 aC = f3(0.0f);
+    float aW = 0.0f;
+    // rows j = -1, 0, 1, 2 of the 12-tap cross; offsets built by additions only
+    const float vxm = vx00 - Bx, vym = vy00 - By;                               // (0,-1)
+    easu_tap_v(aC, aW, vxm, vym, lob, clp, t[-TW]);                              // b (0,-1)
+    easu_tap_v(aC, aW, vxm + Ax, vym + Ay, lob, clp, t[-TW + 1]);                // c (1,-1)
+    easu_tap_v(aC, aW, vx00 - Ax, vy00 - Ay, lob, clp, t[-1]);                   // e (-1,0)
+    easu_tap_v(aC, aW, vx00, vy00, lob, clp, tf);                                // f (0,0)
+    easu_tap_v(aC, aW, vx00 + Ax, vy00 + Ay, lob, clp, tg);                      // g (1,0)
+    easu_tap_v(aC, aW, fmaf(2.0f, Ax, vx00), fmaf(2.0f, Ay, vy00), lob, clp, t[2]);   // h (2,0)
+    const float vx1 = vx00 + Bx, vy1 = vy00 + By;                                // (0,1)
+    easu_tap_v(aC, aW, vx1 - Ax, vy1 - Ay, lob, clp, t[TW - 1]);                 // i (-1,1)
+    easu_tap_v(aC, aW, vx1, vy1, lob, clp, tj);                                  // j (0,1)
+    easu_tap_v(aC, aW, vx1 + Ax, vy1 + Ay, lob, clp, tk);                        // k (1,1)
+    easu_tap_v(aC, aW, fmaf(2.0f, Ax, vx1), fmaf(2.0f, Ay, vy1), lob, clp, t[TW + 2]);   // l (2,1)
+    const float vx2 = fmaf(2.0f, Bx, vx00), vy2 = fmaf(2.0f, By, vy00);          // (0,2)
+    easu_tap_v(aC, aW, vx2, vy2, lob, clp, t[2 * TW]);                           // n (0,2)
+    easu_tap_v(aC, aW, vx2 + Ax, vy2 + Ay, lob, clp, t[2 * TW + 1]);             // o (1,2)
+    const float rw = rcp_fast(aW);
+    return fmin3(max4, fmax3(min4, aC * rw));
+}
+
 template <int ADDR, bool MULTI = false>
 __global__ void __launch_bounds__(EU_BX * EU_BY, EU_BY <= 8 ? 4 : 2) easu_up_kernel(ImgV in, PostOut<MULTI> out, EasuCon con) {
     __shared__ float4 tile[EU_TH][EU_TW];          // rgb + luma
@@ -600,19 +670,7 @@ __global__ void __launch_bounds__(EU_BX * EU_BY, EU_BY <= 8 ? 4 : 2) easu_up_ker
     // ---- phase 1 ----
     {
         const int cx = threadIdx.x, cy = threadIdx.y;
-        if (cx < ncx && cy < ncy) {
-            const float4* t = &tile[cy + 1][cx + 1];                   // 'f'
-            const float bL = t[-EU_TW].w, cL = t[-EU_TW + 1].w;
-            const float eL = t[-1].w, fL = t[0].w, gL = t[1].w, hL = t[2].w;
-            const float iL = t[EU_TW - 1].w, jL = t[EU_TW].w, kL = t[EU_TW + 1].w, lL = t[EU_TW + 2].w;
-            const float nL = t[2 * EU_TW].w, oL = t[2 * EU_TW + 1].w;
-            const EasuSet sS = easu_set_shared(bL, eL, fL, gL, jL), sT = easu_set_shared(cL, fL, gL, hL, kL);
-            const EasuSet sU = easu_set_shared(fL, iL, jL, kL, nL), sV = easu_set_shared(gL, jL, kL, lL, oL);
-            sets[0][cy][cx] = make_float4(sS.dirX, sS.dirY, sS.lenX, sS.lenY);
-            sets[1][cy][cx] = make_float4(sT.dirX, sT.dirY, sT.lenX, sT.lenY);
-            sets[2][cy][cx] = make_float4(sU.dirX, sU.dirY, sU.lenX, sU.lenY);
-            sets[3][cy][cx] = make_float4(sV.dirX, sV.dirY, sV.lenX, sV.lenY);
-        }
+        if (cx < ncx && cy < ncy) easu_up_sets<EU_TW>(&tile[cy + 1][cx + 1], sets[0][cy][cx], sets[1][cy][cx], sets[2][cy][cx], sets[3][cy][cx]);
     }
     __syncthreads();
     // ---- phase 2: one output pixel per thread ----
@@ -622,52 +680,7 @@ __global__ void __launch_bounds__(EU_BX * EU_BY, EU_BY <= 8 ? 4 : 2) easu_up_ker
     const float fpx = floorf(ppx), fpy = floorf(ppy);
     ppx -= fpx; ppy -= fpy;
     const int cx = (int)fpx - fxFirst, cy = (int)fpy - fyFirst;
-    float2 dir = make_float2(0.0f, 0.0f);
-    float len = 0.0f;
-    easu_set_blend(dir, len, (1.0f - ppx) * (1.0f - ppy), sets[0][cy][cx]);
-    easu_set_blend(dir, len, ppx * (1.0f - ppy), sets[1][cy][cx]);
-    easu_set_blend(dir, len, (1.0f - ppx) * ppy, sets[2][cy][cx]);
-    easu_set_blend(dir, len, ppx * ppy, sets[3][cy][cx]);
-    float dirR = dir.x * dir.x + dir.y * dir.y;
-    const bool zro = dirR < (1.0f / 32768.0f);
-    dirR = APrxLoRsqF1(dirR);
-    dirR = zro ? 1.0f : dirR;
-    dir.x = zro ? 1.0f : dir.x;
-    dir.x *= dirR; dir.y *= dirR;
-    len = len * 0.5f;
-    len *= len;
-    const float stretch = (dir.x * dir.x + dir.y * dir.y) * APrxLoRcpF1(fmaxf(fabsf(dir.x), fabsf(dir.y)));
-    const float lenx = fmaf(stretch - 1.0f, len, 1.0f), leny = fmaf(-0.5f, len, 1.0f);
-    const float lob = fmaf((1.0f / 4.0f - 0.04f) - 0.5f, len, 0.5f);
-    const float clp = APrxLoRcpF1(lob);
-    // rotated + scaled offset of tap (i,j):  vx = ((i-ppx)*dir.x + (j-ppy)*dir.y)*lenx,  vy = (-(i-ppx)*dir.y + (j-ppy)*dir.x)*leny
-    const float Ax = dir.x * lenx, Bx = dir.y * lenx;        // d vx / d i , d vx / d j
-    const float Ay = -dir.y * leny, By = dir.x * leny;       // d vy / d i , d vy / d j
-    const float vx00 = -(ppx * Ax + ppy * Bx), vy00 = -(ppx * Ay + ppy * By);
-    const float4* t = &tile[cy + 1][cx + 1];                 // 'f'
-    const float4 tf = t[0], tg = t[1], tj = t[EU_TW], tk = t[EU_TW + 1];
-    const float3 min4 = fmin3(fmin3(xyz(tf), fmin3(xyz(tg), xyz(tj))), xyz(tk));
-    const float3 max4 = fmax3(fmax3(xyz(tf), fmax3(xyz(tg), xyz(tj))), xyz(tk));
-    float3 aC = f3(0.0f);
-    float aW = 0.0f;
-    // rows j = -1, 0, 1, 2 of the 12-tap cross; offsets built by additions only
-    const float vxm = vx00 - Bx, vym = vy00 - By;                               // (0,-1)
-    easu_tap_v(aC, aW, vxm, vym, lob, clp, t[-EU_TW]);                           // b (0,-1)
-    easu_tap_v(aC, aW, vxm + Ax, vym + Ay, lob, clp, t[-EU_TW + 1]);             // c (1,-1)
-    easu_tap_v(aC, aW, vx00 - Ax, vy00 - Ay, lob, clp, t[-1]);                   // e (-1,0)
-    easu_tap_v(aC, aW, vx00, vy00, lob, clp, tf);                                // f (0,0)
-    easu_tap_v(aC, aW, vx00 + Ax, vy00 + Ay, lob, clp, tg);                      // g (1,0)
-    easu_tap_v(aC, aW, fmaf(2.0f, Ax, vx00), fmaf(2.0f, Ay, vy00), lob, clp, t[2]);   // h (2,0)
-    const float vx1 = vx00 + Bx, vy1 = vy00 + By;                                // (0,1)
-    easu_tap_v(aC, aW, vx1 - Ax, vy1 - Ay, lob, clp, t[EU_TW - 1]);              // i (-1,1)
-    easu_tap_v(aC, aW, vx1, vy1, lob, clp, tj);                                  // j (0,1)
-    easu_tap_v(aC, aW, vx1 + Ax, vy1 + Ay, lob, clp, tk);                        // k (1,1)
-    easu_tap_v(aC, aW, fmaf(2.0f, Ax, vx1), fmaf(2.0f, Ay, vy1), lob, clp, t[EU_TW + 2]);   // l (2,1)
-    const float vx2 = fmaf(2.0f, Bx, vx00), vy2 = fmaf(2.0f, By, vy00);          // (0,2)
-    easu_tap_v(aC, aW, vx2, vy2, lob, clp, t[2 * EU_TW]);                        // n (0,2)
-    easu_tap_v(aC, aW, vx2 + Ax, vy2 + Ay, lob, clp, t[2 * EU_TW + 1]);          // o (1,2)
-    const float rw = rcp_fast(aW);
-    const float3 pix = fmin3(max4, fmax3(min4, aC * rw));
+    const float3 pix = easu_up_px<EU_TW>(&tile[cy + 1][cx + 1], sets[0][cy][cx], sets[1][cy][cx], sets[2][cy][cx], sets[3][cy][cx], ppx, ppy);
     store_px(out, x, y, make_float4(pix.x, pix.y, pix.z, 1.0f));
     post_retire(out);
 }
@@ -722,6 +735,58 @@ __device__ __forceinline__ void easu2_tap(EasuAcc2& A, f2 vx, f2 vy, const EasuP
     A.w = A.w + w;
 }
 
+// The quad's shared part for 'f' = t[0] of a staged footprint with row stride TW (rgb + luma): the four FsrEasuSetF analyses and
+// the clamp range of f, g, j, k (ffx_fsr1.h:395-398). The analyses need only the lumas; the colours are re-read from shared
+// memory tap by tap in easu2_row, so that the 12 texels are not live in registers across the whole quad (48 registers: 2 CTAs
+// per SM became 6).
+struct EasuQuad { EasuSet S, T, U, V; float3 min4, max4; };
+template <int TW>
+__device__ __forceinline__ EasuQuad easu2_quad(const float4* t) {
+    EasuQuad q;
+    const float bL = t[-TW].w, cL = t[-TW + 1].w, eL = t[-1].w, hL = t[2].w;
+    const float iL = t[TW - 1].w, lL = t[TW + 2].w, nL = t[2 * TW].w, oL = t[2 * TW + 1].w;
+    const float4 tf = t[0], tg = t[1], tj = t[TW], tk = t[TW + 1];
+    q.S = easu_set_shared(bL, eL, tf.w, tg.w, tj.w); q.T = easu_set_shared(cL, tf.w, tg.w, hL, tk.w);
+    q.U = easu_set_shared(tf.w, iL, tj.w, tk.w, nL); q.V = easu_set_shared(tg.w, tj.w, tk.w, lL, oL);
+    q.min4 = fmin3(fmin3(xyz(tf), fmin3(xyz(tg), xyz(tj))), xyz(tk));
+    q.max4 = fmax3(fmax3(xyz(tf), fmax3(xyz(tg), xyz(tj))), xyz(tk));
+    return q;
+}
+// One output row of the quad (pp.y = ppy: .25 for the upper row, .75 for the lower one): its {left, right} pixels, alpha 1
+template <int TW>
+__device__ __forceinline__ void easu2_row(const float4* t, const EasuQuad& q, float ppy, float4& left, float4& right) {
+    // bilinear weights of the four analyses for {left, right}: (1-ppx)(1-ppy), ppx(1-ppy), (1-ppx)ppy, ppx ppy — exact constants
+    const f2 wS = mk(0.75f * (1.0f - ppy), 0.25f * (1.0f - ppy)), wT = mk(0.25f * (1.0f - ppy), 0.75f * (1.0f - ppy));
+    const f2 wU = mk(0.75f * ppy, 0.25f * ppy), wV = mk(0.25f * ppy, 0.75f * ppy);
+    const EasuPx2 P = easu2_direction(q.S, q.T, q.U, q.V, wS, wT, wU, wV);
+    // rotated + scaled offset of tap (i,j):  vx = ((i-ppx)*dir.x + (j-ppy)*dir.y)*lenx,  vy = (-(i-ppx)*dir.y + (j-ppy)*dir.x)*leny
+    const f2 Ax = P.dirx * P.lenx, Bx = P.diry * P.lenx;         // d vx / d i , d vx / d j
+    const f2 Ay = mk(-P.diry.v.x, -P.diry.v.y) * P.leny, By = P.dirx * P.leny;
+    const f2 nppy = bc(-ppy);
+    const f2 vx00 = fma2(nppy, Bx, mk(-0.25f, -0.75f) * Ax), vy00 = fma2(nppy, By, mk(-0.25f, -0.75f) * Ay);
+    EasuAcc2 A; A.r = A.g = A.b = A.w = bc(0.0f);
+    const f2 vxm = vx00 - Bx, vym = vy00 - By;                                        // (0,-1)
+    easu2_tap(A, vxm, vym, P, t[-TW]);                                                 // b (0,-1)
+    easu2_tap(A, vxm + Ax, vym + Ay, P, t[-TW + 1]);                                   // c (1,-1)
+    easu2_tap(A, vx00 - Ax, vy00 - Ay, P, t[-1]);                                      // e (-1,0)
+    easu2_tap(A, vx00, vy00, P, t[0]);                                                 // f (0,0)
+    easu2_tap(A, vx00 + Ax, vy00 + Ay, P, t[1]);                                       // g (1,0)
+    easu2_tap(A, fma2(bc(2.0f), Ax, vx00), fma2(bc(2.0f), Ay, vy00), P, t[2]);         // h (2,0)
+    const f2 vx1 = vx00 + Bx, vy1 = vy00 + By;                                         // (0,1)
+    easu2_tap(A, vx1 - Ax, vy1 - Ay, P, t[TW - 1]);                                    // i (-1,1)
+    easu2_tap(A, vx1, vy1, P, t[TW]);                                                  // j (0,1)
+    easu2_tap(A, vx1 + Ax, vy1 + Ay, P, t[TW + 1]);                                    // k (1,1)
+    easu2_tap(A, fma2(bc(2.0f), Ax, vx1), fma2(bc(2.0f), Ay, vy1), P, t[TW + 2]);      // l (2,1)
+    const f2 vx2 = fma2(bc(2.0f), Bx, vx00), vy2 = fma2(bc(2.0f), By, vy00);           // (0,2)
+    easu2_tap(A, vx2, vy2, P, t[2 * TW]);                                              // n (0,2)
+    easu2_tap(A, vx2 + Ax, vy2 + Ay, P, t[2 * TW + 1]);                                // o (1,2)
+    const f2 rw = rcp2(A.w);                                                           // ARcpF1 = rcp() in the HLSL
+    const f2 cr = A.r * rw, cg = A.g * rw, cb = A.b * rw;
+    const float3 mn = q.min4, mx = q.max4;
+    left = make_float4(fminf(mx.x, fmaxf(mn.x, cr.v.x)), fminf(mx.y, fmaxf(mn.y, cg.v.x)), fminf(mx.z, fmaxf(mn.z, cb.v.x)), 1.0f);
+    right = make_float4(fminf(mx.x, fmaxf(mn.x, cr.v.y)), fminf(mx.y, fmaxf(mn.y, cg.v.y)), fminf(mx.z, fmaxf(mn.z, cb.v.y)), 1.0f);
+}
+
 template <int ADDR, bool MULTI = false>
 __global__ void __launch_bounds__(E2_BX * E2_BY, E2_MINB) easu_2x_kernel(ImgV in, PostOut<MULTI> out) {
     __shared__ float4 tile[E2_TH][E2_TW];          // rgb + luma
@@ -737,57 +802,17 @@ __global__ void __launch_bounds__(E2_BX * E2_BY, E2_MINB) easu_2x_kernel(ImgV in
     const int ox = 2 * k + 1, oy = 2 * m + 1;                        // top-left pixel of the quad
     if (ox >= out.w || oy >= out.h) { post_retire(out); return; }    // (k, m) beyond the last owning texel
     const float4* t = &tile[threadIdx.y + 1][threadIdx.x + 1];      // 'f'
-    float3 min4, max4;
-    EasuSet S, T, U, V;
-    {   // the four analyses need only the lumas; the colours are re-read from shared memory tap by tap below, so that the 12
-        // texels are not live in registers across the whole kernel (48 registers: 2 CTAs per SM became 6)
-        const float bL = t[-E2_TW].w, cL = t[-E2_TW + 1].w, eL = t[-1].w, hL = t[2].w;
-        const float iL = t[E2_TW - 1].w, lL = t[E2_TW + 2].w, nL = t[2 * E2_TW].w, oL = t[2 * E2_TW + 1].w;
-        const float4 tf = t[0], tg = t[1], tj = t[E2_TW], tk = t[E2_TW + 1];
-        S = easu_set_shared(bL, eL, tf.w, tg.w, tj.w); T = easu_set_shared(cL, tf.w, tg.w, hL, tk.w);
-        U = easu_set_shared(tf.w, iL, tj.w, tk.w, nL); V = easu_set_shared(tg.w, tj.w, tk.w, lL, oL);
-        // clamp range of the quad: min/max of f, g, j, k (ffx_fsr1.h:395-398)
-        min4 = fmin3(fmin3(xyz(tf), fmin3(xyz(tg), xyz(tj))), xyz(tk));
-        max4 = fmax3(fmax3(xyz(tf), fmax3(xyz(tg), xyz(tj))), xyz(tk));
-    }
+    const EasuQuad q = easu2_quad<E2_TW>(t);
     // the two output rows one after the other: one pair's state live at a time
 #pragma unroll 1
     for (int row = 0; row < 2; ++row) {                              // output rows oy (pp.y = .25) and oy+1 (pp.y = .75)
-        const float ppy = row ? 0.75f : 0.25f;
         const int y = oy + row;
         if (y < 0 || y >= out.h) continue;
-        // bilinear weights of the four analyses for {left, right}: (1-ppx)(1-ppy), ppx(1-ppy), (1-ppx)ppy, ppx ppy — exact constants
-        const f2 wS = mk(0.75f * (1.0f - ppy), 0.25f * (1.0f - ppy)), wT = mk(0.25f * (1.0f - ppy), 0.75f * (1.0f - ppy));
-        const f2 wU = mk(0.75f * ppy, 0.25f * ppy), wV = mk(0.25f * ppy, 0.75f * ppy);
-        const EasuPx2 P = easu2_direction(S, T, U, V, wS, wT, wU, wV);
-        // rotated + scaled offset of tap (i,j):  vx = ((i-ppx)*dir.x + (j-ppy)*dir.y)*lenx,  vy = (-(i-ppx)*dir.y + (j-ppy)*dir.x)*leny
-        const f2 Ax = P.dirx * P.lenx, Bx = P.diry * P.lenx;         // d vx / d i , d vx / d j
-        const f2 Ay = mk(-P.diry.v.x, -P.diry.v.y) * P.leny, By = P.dirx * P.leny;
-        const f2 nppy = bc(-ppy);
-        const f2 vx00 = fma2(nppy, Bx, mk(-0.25f, -0.75f) * Ax), vy00 = fma2(nppy, By, mk(-0.25f, -0.75f) * Ay);
-        EasuAcc2 A; A.r = A.g = A.b = A.w = bc(0.0f);
-        const f2 vxm = vx00 - Bx, vym = vy00 - By;                                        // (0,-1)
-        easu2_tap(A, vxm, vym, P, t[-E2_TW]);                                                     // b (0,-1)
-        easu2_tap(A, vxm + Ax, vym + Ay, P, t[-E2_TW + 1]);                                           // c (1,-1)
-        easu2_tap(A, vx00 - Ax, vy00 - Ay, P, t[-1]);                                         // e (-1,0)
-        easu2_tap(A, vx00, vy00, P, t[0]);                                                   // f (0,0)
-        easu2_tap(A, vx00 + Ax, vy00 + Ay, P, t[1]);                                         // g (1,0)
-        easu2_tap(A, fma2(bc(2.0f), Ax, vx00), fma2(bc(2.0f), Ay, vy00), P, t[2]);           // h (2,0)
-        const f2 vx1 = vx00 + Bx, vy1 = vy00 + By;                                         // (0,1)
-        easu2_tap(A, vx1 - Ax, vy1 - Ay, P, t[E2_TW - 1]);                                           // i (-1,1)
-        easu2_tap(A, vx1, vy1, P, t[E2_TW]);                                                     // j (0,1)
-        easu2_tap(A, vx1 + Ax, vy1 + Ay, P, t[E2_TW + 1]);                                           // k (1,1)
-        easu2_tap(A, fma2(bc(2.0f), Ax, vx1), fma2(bc(2.0f), Ay, vy1), P, t[E2_TW + 2]);             // l (2,1)
-        const f2 vx2 = fma2(bc(2.0f), Bx, vx00), vy2 = fma2(bc(2.0f), By, vy00);           // (0,2)
-        easu2_tap(A, vx2, vy2, P, t[2 * E2_TW]);                                                     // n (0,2)
-        easu2_tap(A, vx2 + Ax, vy2 + Ay, P, t[2 * E2_TW + 1]);                                           // o (1,2)
-        const f2 rw = rcp2(A.w);                                                           // ARcpF1 = rcp() in the HLSL
-        const f2 cr = A.r * rw, cg = A.g * rw, cb = A.b * rw;
+        float4 left, right;
+        easu2_row<E2_TW>(t, q, row ? 0.75f : 0.25f, left, right);
         float4* dst = out_row(out, y);
-        if (ox >= 0) store_px(out, dst + ox, ox, y, make_float4(fminf(max4.x, fmaxf(min4.x, cr.v.x)), fminf(max4.y, fmaxf(min4.y, cg.v.x)),
-                                                      fminf(max4.z, fmaxf(min4.z, cb.v.x)), 1.0f));
-        if (ox + 1 < out.w) store_px(out, dst + ox + 1, ox + 1, y, make_float4(fminf(max4.x, fmaxf(min4.x, cr.v.y)), fminf(max4.y, fmaxf(min4.y, cg.v.y)),
-                                                                     fminf(max4.z, fmaxf(min4.z, cb.v.y)), 1.0f));
+        if (ox >= 0) store_px(out, dst + ox, ox, y, left);
+        if (ox + 1 < out.w) store_px(out, dst + ox + 1, ox + 1, y, right);
     }
     post_retire(out);
 }
@@ -961,6 +986,294 @@ extern "C" int vq_fsr_easu_source_rows(const uint32_t con[16], int address_mode,
     VQ_REQUIRE(vqeasu::axis_ok(c.c0y, c.c0w, in_height, out_height),
                "easu: con0 puts taps outside [-h, 2h) of the input (constants not built for these heights?)");
     return vqeasu::source_rows(c.c0y, c.c0w, address_mode == VQ_ADDRESS_WRAP, in_height, row_begin, row_end, ranges);
+}
+
+// =============================================================================================
+// RenderPostProcess in one launch (vq_post_process): the tonemapper fused into FSR1 EASU + RCAS, or into CAS
+// =============================================================================================
+// Each CTA owns a tile of the display frame. It stages the EASU (or CAS) input footprint of the tile TONEMAPPED (tonemap_px on
+// the texel the sampler's WRAP / CLAMP fold selects, i.e. the texel of vq_tonemap's output that EASU would read), runs EASU on
+// the tile plus the 1-pixel ring RCAS reads, keeps those pixels in shared memory and runs RCAS from there. Ring pixels outside
+// the display frame are 0, as rcas_kernel's load_zero_border reads them. Every pixel is computed by the device functions of the
+// single-pass kernels from the same values, so the display frame equals vq_tonemap -> vq_fsr_easu -> vq_fsr_rcas bit for bit.
+// The ring is recomputed by each CTA (the measured choice, DESIGN.md §9): 64 x 16 EASU pixels per 62 x 14 tile on the 2x path,
+// 32 x 16 per 30 x 14 on the up path.
+
+// The tonemapper's variants as tonemap_launch selects them; the fused kernels take the variant as a uniform run-time value
+// (one instantiation per variant would multiply their number by six)
+enum { TMV_SRGB_GAMMA = 0, TMV_SRGB, TMV_PQ_709, TMV_PQ_2020, TMV_LINEAR, TMV_UNKNOWN };
+static int tonemap_variant(const VqTonemapperParams* p) {
+    switch (p->OutputDisplayCurve) {
+        case VQ_DISPLAY_CURVE_SRGB: return p->ToggleGammaCorrection ? TMV_SRGB_GAMMA : TMV_SRGB;
+        case VQ_DISPLAY_CURVE_ST2084: return p->ContentColorSpace == VQ_COLOR_SPACE_REC_709 ? TMV_PQ_709 : TMV_PQ_2020;
+        case VQ_DISPLAY_CURVE_LINEAR: return TMV_LINEAR;
+        default: return TMV_UNKNOWN;
+    }
+}
+__device__ __forceinline__ float4 tonemap_var(int v, float4 c, float hdrScalar) {
+    switch (v) {
+        case TMV_SRGB_GAMMA: return tonemap_px<VQ_DISPLAY_CURVE_SRGB, true, false>(c, hdrScalar);
+        case TMV_SRGB:       return tonemap_px<VQ_DISPLAY_CURVE_SRGB, false, false>(c, hdrScalar);
+        case TMV_PQ_709:     return tonemap_px<VQ_DISPLAY_CURVE_ST2084, false, true>(c, hdrScalar);
+        case TMV_PQ_2020:    return tonemap_px<VQ_DISPLAY_CURVE_ST2084, false, false>(c, hdrScalar);
+        case TMV_LINEAR:     return tonemap_px<VQ_DISPLAY_CURVE_LINEAR, false, false>(c, hdrScalar);
+        default:             return tonemap_px<3, false, false>(c, hdrScalar);
+    }
+}
+struct TonemapArg { int variant; float hdrScalar; };
+static TonemapArg tonemap_arg(const VqTonemapperParams* p) {
+    TonemapArg t; t.variant = tonemap_variant(p); t.hdrScalar = p->DisplayReferenceBrightnessLevel / 10000.0f;   // as tonemap_launch
+    return t;
+}
+
+// EASU's staged texel (rgb + luma) of the tonemapped image at tap (x, y)
+template <int ADDR>
+__device__ __forceinline__ float4 tonemapped_tap(const ImgV& in, int x, int y, TonemapArg tm) {
+    const float3 c = load_addr<ADDR>(in, x, y);
+    const float4 v = tonemap_var(tm.variant, make_float4(c.x, c.y, c.z, 0.0f), tm.hdrScalar);
+    return make_float4(v.x, v.y, v.z, luma2(xyz(v)));
+}
+
+// RCAS over the CTA's display tile at (X0, Y0) from the EASU pixels e[ly][lx] = display (X0 - 1 + lx, Y0 - 1 + ly)
+template <int EW, int EH, class Out>
+__device__ __forceinline__ void rcas_from_shared(const float4 (*e)[EW], int X0, int Y0, const Out& out, float sharp) {
+    constexpr int TX = EW - 2, TY = EH - 2;
+    for (int i = threadIdx.y * blockDim.x + threadIdx.x; i < TX * TY; i += blockDim.x * blockDim.y) {
+        const int ly = i / TX, lx = i - ly * TX;
+        const int x = X0 + lx, y = Y0 + ly;
+        if (x >= out.w || y >= out.h) continue;
+        const float4* c = &e[ly + 1][lx + 1];
+        const float3 o = rcas_px(xyz(c[-EW]), xyz(c[-1]), xyz(c[0]), xyz(c[1]), xyz(c[EW]), sharp);
+        store_px(out, x, y, make_float4(o.x, o.y, o.z, 1.0f));
+    }
+}
+
+// ---- exact 2x: one thread per 'f' texel owning a 2x2 output quad, as easu_2x_kernel --------------------------------------------
+// Quad (k, m) covers display (2k+1 .. 2k+2, 2m+1 .. 2m+2): the CTA's 32 x 8 quads cover 64 x 16 EASU pixels, the 62 x 14 display
+// tile and its ring exactly.
+constexpr int PF2_QX = 32, PF2_QY = 8;                          // quads per CTA, one per thread
+constexpr int PF2_TX = 2 * PF2_QX - 2, PF2_TY = 2 * PF2_QY - 2; // display tile
+constexpr int PF2_SW = PF2_QX + 3, PF2_SH = PF2_QY + 3;         // staged footprint: texels k-1 .. k+2, m-1 .. m+2
+
+template <int ADDR, bool MULTI = false>
+__global__ void __launch_bounds__(PF2_QX * PF2_QY, 1024 / (PF2_QX * PF2_QY)) post_fsr2x_kernel(ImgV in, PostOut<MULTI> out, TonemapArg tm, float sharp) {
+    __shared__ float4 tile[PF2_SH][PF2_SW];                      // tonemapped rgb + luma
+    __shared__ float4 eo[2 * PF2_QY][2 * PF2_QX];                // EASU output at display (X0 - 1 + lx, Y0 - 1 + ly); 0 outside
+    const int X0 = (int)blockIdx.x * PF2_TX, Y0 = (int)tile_row(out) * PF2_TY;
+    const int k0 = X0 / 2 - 1, m0 = Y0 / 2 - 1;
+    for (int i = threadIdx.y * PF2_QX + threadIdx.x; i < PF2_SH * PF2_SW; i += PF2_QX * PF2_QY) {
+        const int ly = i / PF2_SW, lx = i - ly * PF2_SW;
+        const int x = k0 - 1 + lx, y = m0 - 1 + ly;
+        // the quads inside the display have k <= in.w - 1, m <= in.h - 1: their taps end at in.w + 1, in.h + 1 (inside the range
+        // load_addr folds); texels beyond are never read
+        if (x <= in.w + 1 && y <= in.h + 1) tile[ly][lx] = tonemapped_tap<ADDR>(in, x, y, tm);
+    }
+    __syncthreads();
+    {
+        const int ox = 2 * (k0 + (int)threadIdx.x) + 1, oy = 2 * (m0 + (int)threadIdx.y) + 1;   // top-left pixel of the quad
+        const bool inside = ox < out.w && oy < out.h;                                            // ox, oy >= -1
+        const float4* t = &tile[threadIdx.y + 1][threadIdx.x + 1];                              // 'f'
+        EasuQuad q;
+        if (inside) q = easu2_quad<PF2_SW>(t);
+#pragma unroll 1
+        for (int row = 0; row < 2; ++row) {
+            const int y = oy + row;
+            float4 left = make_float4(0.0f, 0.0f, 0.0f, 0.0f), right = left;
+            if (inside && y >= 0 && y < out.h) {
+                float4 l, r;
+                easu2_row<PF2_SW>(t, q, row ? 0.75f : 0.25f, l, r);
+                if (ox >= 0) left = l;
+                if (ox + 1 < out.w) right = r;
+            }
+            eo[2 * threadIdx.y + row][2 * threadIdx.x] = left;
+            eo[2 * threadIdx.y + row][2 * threadIdx.x + 1] = right;
+        }
+    }
+    __syncthreads();
+    rcas_from_shared<2 * PF2_QX, 2 * PF2_QY>(eo, X0, Y0, out, sharp);
+    post_retire(out);
+}
+
+// ---- upscaling path (ratio <= 1): easu_up_kernel's two phases on the display tile + ring ----------------------------------------
+constexpr int PFU_EX = 32, PFU_EY = 16;                          // EASU pixels per CTA: the display tile + ring
+constexpr int PFU_TX = PFU_EX - 2, PFU_TY = PFU_EY - 2;          // display tile
+constexpr int PFU_BX = 32, PFU_BY = 8;                           // threads
+constexpr int PFU_CX = vqeasu::FUSED_UP_TILE.cap_x, PFU_CY = vqeasu::FUSED_UP_TILE.cap_y;   // candidate 'f' texels
+constexpr int PFU_SW = PFU_CX + 3, PFU_SH = PFU_CY + 3;          // staged footprint
+static_assert(PFU_TX == vqeasu::FUSED_UP_TILE.x && PFU_TY == vqeasu::FUSED_UP_TILE.y && vqeasu::FUSED_UP_TILE.ring == 1,
+              "vq_post_process's footprint check must describe this kernel's tiling");
+static_assert(PFU_EY == 2 * PFU_BY && PFU_EX == PFU_BX && PFU_CX == PFU_BX, "two EASU pixels and at most two candidates per thread");
+
+template <int ADDR, bool MULTI = false>
+__global__ void __launch_bounds__(PFU_BX * PFU_BY, 4) post_fsr_up_kernel(ImgV in, PostOut<MULTI> out, EasuCon con, TonemapArg tm,
+                                                                          float sharp) {
+    __shared__ float4 tile[PFU_SH][PFU_SW];                      // tonemapped rgb + luma
+    __shared__ float4 sets[4][PFU_CY][PFU_CX];                   // S,T,U,V analyses; then the EASU output (below)
+    const int X0 = (int)blockIdx.x * PFU_TX, Y0 = (int)tile_row(out) * PFU_TY;
+    // EASU runs on display [X0 - 1, X0 + PFU_TX] x [Y0 - 1, Y0 + PFU_TY] clipped to the display: its candidate texels
+    const int ex0 = max(X0 - 1, 0), ey0 = max(Y0 - 1, 0);
+    const int ex1 = min(X0 + PFU_TX, out.w - 1), ey1 = min(Y0 + PFU_TY, out.h - 1);
+    const int fxFirst = (int)floorf(easu_pos(ex0, con.c0x, con.c0z)), fyFirst = (int)floorf(easu_pos(ey0, con.c0y, con.c0w));
+    const int ncx = (int)floorf(easu_pos(ex1, con.c0x, con.c0z)) - fxFirst + 1;
+    const int ncy = (int)floorf(easu_pos(ey1, con.c0y, con.c0w)) - fyFirst + 1;
+    const int sw = ncx + 3, tid = threadIdx.y * PFU_BX + threadIdx.x;
+    for (int i = tid; i < sw * (ncy + 3); i += PFU_BX * PFU_BY) {
+        const int ly = i / sw, lx = i - ly * sw;
+        tile[ly][lx] = tonemapped_tap<ADDR>(in, fxFirst - 1 + lx, fyFirst - 1 + ly, tm);
+    }
+    __syncthreads();
+    // ---- phase 1: the analyses of every candidate ----
+    for (int cy = threadIdx.y; cy < ncy; cy += PFU_BY)
+        if ((int)threadIdx.x < ncx)
+            easu_up_sets<PFU_SW>(&tile[cy + 1][threadIdx.x + 1], sets[0][cy][threadIdx.x], sets[1][cy][threadIdx.x],
+                                 sets[2][cy][threadIdx.x], sets[3][cy][threadIdx.x]);
+    __syncthreads();
+    // ---- phase 2: EASU pixels (tx, ty) and (tx, ty + 8) of the widened tile ----
+    float3 px[2];
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+        const int x = X0 - 1 + (int)threadIdx.x, y = Y0 - 1 + (int)threadIdx.y + r * PFU_BY;
+        px[r] = f3(0.0f);
+        if (x < 0 || y < 0 || x >= out.w || y >= out.h) continue;
+        float ppx = easu_pos(x, con.c0x, con.c0z), ppy = easu_pos(y, con.c0y, con.c0w);
+        const float fpx = floorf(ppx), fpy = floorf(ppy);
+        ppx -= fpx; ppy -= fpy;
+        const int cx = (int)fpx - fxFirst, cy = (int)fpy - fyFirst;
+        px[r] = easu_up_px<PFU_SW>(&tile[cy + 1][cx + 1], sets[0][cy][cx], sets[1][cy][cx], sets[2][cy][cx], sets[3][cy][cx], ppx, ppy);
+    }
+    __syncthreads();                                             // every analysis read: sets[0] becomes the EASU output
+    float4 (*eo)[PFU_EX] = reinterpret_cast<float4 (*)[PFU_EX]>(&sets[0][0][0]);
+    static_assert(PFU_EX * PFU_EY <= PFU_CX * PFU_CY, "the EASU output fits in sets[0]");
+#pragma unroll
+    for (int r = 0; r < 2; ++r) eo[threadIdx.y + r * PFU_BY][threadIdx.x] = make_float4(px[r].x, px[r].y, px[r].z, 0.0f);
+    __syncthreads();
+    rcas_from_shared<PFU_EX, PFU_EY>(eo, X0, Y0, out, sharp);
+    post_retire(out);
+}
+
+// ---- tonemapper -> CAS: the tonemapped 34 x 10 footprint of a 32 x 8 tile in shared memory, 0 outside the image ----------------
+template <bool MULTI = false>
+__global__ void __launch_bounds__(ST_BX * ST_BY) post_cas_kernel(ImgV in, PostOut<MULTI> out, TonemapArg tm, float peak) {
+    __shared__ float4 t[ST_BY + 2][ST_BX + 2];
+    const int X0 = blockIdx.x * ST_BX, Y0 = tile_row(out) * ST_BY;
+    for (int i = threadIdx.y * ST_BX + threadIdx.x; i < (ST_BY + 2) * (ST_BX + 2); i += ST_BX * ST_BY) {
+        const int ly = i / (ST_BX + 2), lx = i - ly * (ST_BX + 2);
+        const int x = X0 - 1 + lx, y = Y0 - 1 + ly;
+        t[ly][lx] = (unsigned)x < (unsigned)in.w && (unsigned)y < (unsigned)in.h ? tonemap_var(tm.variant, __ldg(in.row(y) + x), tm.hdrScalar)
+                                                                                 : make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+    }
+    __syncthreads();
+    const int x = X0 + threadIdx.x, y = Y0 + threadIdx.y;
+    if (x < out.w && y < out.h) {
+        const int lx = threadIdx.x + 1, ly = threadIdx.y + 1;
+        const float3 o = cas_px(xyz(t[ly - 1][lx]), xyz(t[ly][lx - 1]), xyz(t[ly][lx]), xyz(t[ly][lx + 1]), xyz(t[ly + 1][lx]), peak);
+        store_px(out, x, y, make_float4(o.x, o.y, o.z, 1.0f));
+    }
+    post_retire(out);
+}
+
+// The checks vq_post_process and vq_post_process_multi_signal share, before the device is touched. W x H is the display size.
+// Fills `plan`: which branch of RenderPostProcess runs, EASU's path and constants.
+struct PostPlan { bool fsr, cas; vqeasu::Path path; EasuCon con; };
+static int post_process_check(const VqTonemapperParams* tonemapper, const uint32_t cas_const[8], const uint32_t easu_const[16],
+                              int address_mode, const uint32_t rcas_const[4], VqImage scene, int W, int H, PostPlan& plan) {
+    VQ_REQUIRE(tonemapper, "params is null");
+    VQ_REQUIRE(vq_image_ok(scene), "bad image descriptor");
+    VQ_REQUIRE(!easu_const == !rcas_const, "post_process: easu_const and rcas_const are given together or not at all");
+    plan.fsr = easu_const != nullptr;
+    plan.cas = !plan.fsr && cas_const != nullptr;
+    plan.path = vqeasu::EASU_GENERIC;
+    memset(&plan.con, 0, sizeof(plan.con));
+    if (!plan.fsr) {
+        VQ_REQUIRE(W == scene.width && H == scene.height, plan.cas ? "cas: sharpen-only path needs equal sizes (FFXCAS_NO_UPSCALING)"
+                                                                   : "tonemap: in/out size mismatch");
+        return VQ_OK;
+    }
+    VQ_REQUIRE(address_mode == VQ_ADDRESS_WRAP || address_mode == VQ_ADDRESS_CLAMP, "easu: unknown address mode");
+    memcpy(&plan.con, easu_const, 16);
+    const float c0[4] = {plan.con.c0x, plan.con.c0y, plan.con.c0z, plan.con.c0w};
+    const vqeasu::Verdict v = vqeasu::check(c0, scene.width, scene.height, W, H, nullptr, nullptr, vqeasu::FUSED_UP_TILE);
+    VQ_REQUIRE(v != vqeasu::EASU_NONFINITE, "easu: con0 is not finite");
+    VQ_REQUIRE(v != vqeasu::EASU_TAPS_OUTSIDE, "easu: con0 puts taps outside [-w, 2w) x [-h, 2h) of the input (constants not built for these images?)");
+    VQ_REQUIRE(v != vqeasu::EASU_TILE_FOOTPRINT, "post_process: con0 needs more than 32x16 input texels per 30x14 display tile and its ring");
+    plan.path = vqeasu::path(c0, scene.width, scene.height, W, H);
+    VQ_REQUIRE(plan.path != vqeasu::EASU_GENERIC,
+               "post_process: con0 is on EASU's downscaling path (no FsrEasuCon upscale builds it): run vq_tonemap, vq_fsr_easu, vq_fsr_rcas");
+    return VQ_OK;
+}
+
+// Launch geometry of a plan: tile size and count along x and y
+struct PostGrid { int tx, ty, nx, ny; };
+static PostGrid post_grid(const PostPlan& plan, int W, int H) {
+    PostGrid g;
+    if (plan.fsr && plan.path == vqeasu::EASU_2X) { g.tx = PF2_TX; g.ty = PF2_TY; }
+    else if (plan.fsr) { g.tx = PFU_TX; g.ty = PFU_TY; }
+    else if (plan.cas) { g.tx = ST_BX; g.ty = ST_BY; }
+    else { g.tx = TM_THREADS * TM_PX; g.ty = 1; }
+    g.nx = (W + g.tx - 1) / g.tx; g.ny = (H + g.ty - 1) / g.ty;
+    return g;
+}
+
+template <bool MULTI>
+static int post_launch(const PostPlan& plan, const VqTonemapperParams* p, const uint32_t cas_const[8], const uint32_t rcas_const[4],
+                       int address_mode, dim3 grid, ImgV vi, const PostOut<MULTI>& vo, cudaStream_t st) {
+    const TonemapArg tm = tonemap_arg(p);
+    const bool wrap = address_mode == VQ_ADDRESS_WRAP;
+    if (plan.fsr) {
+        float sharp; memcpy(&sharp, &rcas_const[0], 4);
+        if (plan.path == vqeasu::EASU_2X) {
+            if (wrap) post_fsr2x_kernel<VQ_ADDRESS_WRAP, MULTI><<<grid, dim3(PF2_QX, PF2_QY), 0, st>>>(vi, vo, tm, sharp);
+            else      post_fsr2x_kernel<VQ_ADDRESS_CLAMP, MULTI><<<grid, dim3(PF2_QX, PF2_QY), 0, st>>>(vi, vo, tm, sharp);
+        } else {
+            if (wrap) post_fsr_up_kernel<VQ_ADDRESS_WRAP, MULTI><<<grid, dim3(PFU_BX, PFU_BY), 0, st>>>(vi, vo, plan.con, tm, sharp);
+            else      post_fsr_up_kernel<VQ_ADDRESS_CLAMP, MULTI><<<grid, dim3(PFU_BX, PFU_BY), 0, st>>>(vi, vo, plan.con, tm, sharp);
+        }
+        return vq_check_launch(MULTI ? "post_process_multi (fsr)" : "post_process (fsr)");
+    }
+    if (plan.cas) {
+        float peak; memcpy(&peak, &cas_const[4], 4);     // const1.x
+        post_cas_kernel<MULTI><<<grid, dim3(ST_BX, ST_BY), 0, st>>>(vi, vo, tm, peak);
+        return vq_check_launch(MULTI ? "post_process_multi (cas)" : "post_process (cas)");
+    }
+    tonemap_launch<MULTI>(p, grid, vi, vo, st);
+    return vq_check_launch(MULTI ? "post_process_multi (tonemap)" : "post_process (tonemap)");
+}
+
+extern "C" int vq_post_process(VqContext* ctx, const VqTonemapperParams* tonemapper, const uint32_t cas_const[8],
+                               const uint32_t easu_const[16], int address_mode, const uint32_t rcas_const[4], VqImage scene_color,
+                               VqImage display, void* stream) {
+    VQ_REQUIRE(vq_image_ok(display), "bad image descriptor");
+    PostPlan plan;
+    int rc = post_process_check(tonemapper, cas_const, easu_const, address_mode, rcas_const, scene_color, display.width, display.height,
+                                plan); if (rc) return rc;
+    VQ_REQUIRE(!(plan.fsr || plan.cas) || scene_color.ptr != display.ptr, "post_process: in-place is not supported with EASU/RCAS or CAS");
+    rc = vq_enter(ctx); if (rc) return rc;
+    VQ_MARK("PostProcess");
+    const PostGrid g = post_grid(plan, display.width, display.height);
+    return post_launch<false>(plan, tonemapper, cas_const, rcas_const, address_mode, dim3(g.nx, g.ny), make_view(scene_color),
+                              make_view(display), (cudaStream_t)stream);
+}
+
+extern "C" int vq_post_process_multi_signal(VqContext* ctx, const VqTonemapperParams* tonemapper, const uint32_t cas_const[8],
+                                            const uint32_t easu_const[16], int address_mode, const uint32_t rcas_const[4],
+                                            VqImage scene_color, const VqImage* outs, int n_outs, int row_begin, int row_end,
+                                            const VqPeerSignal* signal, void* stream) {
+    VQ_REQUIRE(outs, "null destination list");
+    VQ_REQUIRE(n_outs >= 1 && n_outs <= 8, "1..8 destinations");
+    const int W = outs[0].width, H = outs[0].height;
+    PostPlan plan;
+    int rc = post_process_check(tonemapper, cas_const, easu_const, address_mode, rcas_const, scene_color, W, H, plan); if (rc) return rc;
+    PostDests d;
+    rc = post_dests_check(scene_color, outs, n_outs, W, H, "every destination must have the size of the first",
+                          plan.fsr || plan.cas ? "post_process: in-place is not supported with EASU/RCAS or CAS" : nullptr,
+                          row_begin, row_end, signal, d); if (rc) return rc;
+    rc = vq_enter(ctx); if (rc) return rc;
+    VQ_MARK("PostProcess");
+    if (row_begin == row_end) return VQ_OK;
+    const PostGrid g = post_grid(plan, W, H);
+    const unsigned gy = post_tile_rows(ctx, d, g.ty, 0, g.ty - 1, g.ny);
+    return post_launch<true>(plan, tonemapper, cas_const, rcas_const, address_mode, dim3(g.nx, gy), make_view(scene_color), d,
+                             (cudaStream_t)stream);
 }
 
 // =============================================================================================

@@ -152,8 +152,8 @@ bool VQRenderer::LoadDefaultResources() {
     return cudaStreamSynchronize(nullptr) == cudaSuccess;
 }
 bool VQRenderer::OnWindowSizeChanged(int rw, int rh, int dw, int dh) {
-    return mSceneColor.Create(rw, rh) && mBlurTemp.Create(rw, rh) && mBlurOut.Create(rw, rh) && mTonemapperOut.Create(rw, rh) &&
-           mCASOut.Create(rw, rh) && mEASUOut.Create(dw, dh) && mRCASOut.Create(dw, dh) && vq_ctx_resize(mCtx, rw, rh) == VQ_OK;
+    return mSceneColor.Create(rw, rh) && mBlurTemp.Create(rw, rh) && mBlurOut.Create(rw, rh) && mPostOut.Create(rw, rh) &&
+           mRCASOut.Create(dw, dh) && vq_ctx_resize(mCtx, rw, rh) == VQ_OK;
 }
 
 bool VQRenderer::PreFilterEnvironmentMap(FEnvironmentMapRenderingResources& env, float DiffuseIntegrationStep) {
@@ -326,24 +326,17 @@ const VqImage* VQRenderer::RenderPostProcess(cudaStream_t pCmd, const FPostProce
         if (vq_gaussian_blur_y(mCtx, &bp, mBlurTemp.View(), mBlurOut.View(), pCmd) != VQ_OK) return fail("vq_gaussian_blur_y");
         colorIn = mBlurOut.View();
     }
-    {                                                                      // "TonemapperCS" SceneRendering.cpp:2640-2656
-        VqTonemapperParams tp{(int)PPParams.TonemapperParams.ContentColorSpace, (int)PPParams.TonemapperParams.OutputDisplayCurve,
-                              PPParams.TonemapperParams.DisplayReferenceBrightnessLevel, PPParams.TonemapperParams.ToggleGammaCorrection,
-                              PPParams.TonemapperParams.UIHDRBrightness};
-        if (vq_tonemap(mCtx, &tp, colorIn, mTonemapperOut.View(), pCmd) != VQ_OK) return fail("vq_tonemap");
-        mLastOutput = mTonemapperOut.View();
-    }
-    if (PPParams.IsFFXCASEnabled() && PPParams.Sharpness > 0.0f) {         // "FFX-CAS CS" SceneRendering.cpp:2658-2693
-        if (vq_cas(mCtx, PPParams.FFXCASParams.CASConstantBlock, mTonemapperOut.View(), mCASOut.View(), pCmd) != VQ_OK) return fail("vq_cas");
-        mLastOutput = mCASOut.View();
-    }
-    if (PPParams.IsFSREnabled()) {                                         // SceneRendering.cpp:2695-2783
-        if (vq_fsr_easu(mCtx, PPParams.FSR_EASUParams.EASUConstantBlock, VQ_ADDRESS_WRAP, mTonemapperOut.View(), mEASUOut.View(), pCmd) != VQ_OK)
-            return fail("vq_fsr_easu");
-        if (vq_fsr_rcas(mCtx, PPParams.FSR_RCASParams.RCASConstantBlock, mEASUOut.View(), mRCASOut.View(), pCmd) != VQ_OK)
-            return fail("vq_fsr_rcas");
-        mLastOutput = mRCASOut.View();
-    }
+    // "TonemapperCS" (SceneRendering.cpp:2640-2656), then "FFX-CAS CS" (2658-2693) or "FSR-EASU CS" + "FSR-RCAS CS" (2695-2783):
+    // one launch, no intermediate images
+    const VqTonemapperParams tp{(int)PPParams.TonemapperParams.ContentColorSpace, (int)PPParams.TonemapperParams.OutputDisplayCurve,
+                                PPParams.TonemapperParams.DisplayReferenceBrightnessLevel, PPParams.TonemapperParams.ToggleGammaCorrection,
+                                PPParams.TonemapperParams.UIHDRBrightness};
+    const bool bFSR = PPParams.IsFSREnabled(), bCAS = PPParams.IsFFXCASEnabled() && PPParams.Sharpness > 0.0f;
+    mLastOutput = bFSR ? mRCASOut.View() : mPostOut.View();
+    if (vq_post_process(mCtx, &tp, bCAS ? PPParams.FFXCASParams.CASConstantBlock : nullptr,
+                        bFSR ? PPParams.FSR_EASUParams.EASUConstantBlock : nullptr, VQ_ADDRESS_WRAP,
+                        bFSR ? PPParams.FSR_RCASParams.RCASConstantBlock : nullptr, colorIn, mLastOutput, pCmd) != VQ_OK)
+        return fail("vq_post_process");
     return &mLastOutput;                                                   // "return pRscOutput" SceneRendering.cpp:2787
 }
 

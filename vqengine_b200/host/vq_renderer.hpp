@@ -268,7 +268,9 @@ private:
                             const FGraphicsSettings& GFXSettings, bool bHDR, VqPerFrameData& PerFrame, VqPerViewLightingData& PerView) const;
     VqContext* mCtx = nullptr;
     FTexture2D mBRDFLUT;                                        // EProceduralTextures::IBL_BRDF_INTEGRATION_LUT
-    FTexture2D mSceneColor, mBlurTemp, mBlurOut, mTonemapperOut, mCASOut, mEASUOut, mRCASOut;
+    FTexture2D mSceneColor, mBlurTemp, mBlurOut;
+    FTexture2D mPostOut;                                        // RenderPostProcess's output without FSR (render size)
+    FTexture2D mRCASOut;                                        // ... with FSR (display size)
     VqImage mLastOutput{};
 };
 
