@@ -133,6 +133,14 @@ def specular_probe(env, max_lod, n_uniform, seed, offset=0.0):
     nrm = np.concatenate([N, r[:, None]], 1)
     alb = np.ones((n, 4), np.float32)
     planes, idx = _frame([pos, nrm, alb])
+    pf, pv = constants(cam, max_lod, offset)
+    want, tol = specular_expect(env, planes, cam, max_lod, offset)
+    return dict(planes=planes, pf=pf, pv=pv, want=want, tol=tol)
+
+
+def specular_expect(env, planes, cam, max_lod, offset=0.0):
+    """the specular probe's float64 value and bound, from the G-buffer planes the kernel reads"""
+    res, mips = env["spec_res"], env["spec_mips"]
     V = _v64(planes[0][..., :3].reshape(-1, 3), cam)
     Nf = planes[1][..., :3].reshape(-1, 3).astype(np.float64)
     rf = planes[1][..., 3].ravel()
@@ -144,9 +152,7 @@ def specular_probe(env, max_lod, n_uniform, seed, offset=0.0):
     rel = 2.0 ** -19 * (1.0 + 2.0 * (Nf * Nf).sum(1)) / np.linalg.norm(R, axis=1)
     span = float(env["spec"].max() - env["spec"].min())
     tol = _cube_tol((res >> mip).astype(np.float64), rel, span) + 4 * U24 * np.abs(want).max(1)
-    pf, pv = constants(cam, max_lod, offset)
-    return dict(planes=planes, pf=pf, pv=pv, want=want.reshape(planes[0].shape[:2] + (3,)),
-                tol=tol.reshape(planes[0].shape[:2]))
+    return want.reshape(planes[0].shape[:2] + (3,)), tol.reshape(planes[0].shape[:2])
 
 
 def diffuse_probe(env, n_uniform, seed, offset=0.0, max_lod=5):
@@ -165,15 +171,21 @@ def diffuse_probe(env, n_uniform, seed, offset=0.0, max_lod=5):
     nrm = np.concatenate([N, np.ones((n, 1), np.float32)], 1)
     alb = np.concatenate([np.ones((n, 3), np.float32), np.zeros((n, 1), np.float32)], 1)
     planes, _ = _frame([pos, nrm, alb])
+    pf, pv = constants(cam, max_lod, offset)
+    want, tol = diffuse_expect(env, planes, offset)
+    return dict(planes=planes, pf=pf, pv=pv, want=want, tol=tol)
+
+
+def diffuse_expect(env, planes, offset=0.0):
+    """the diffuse probe's float64 value and bound, from the G-buffer planes the kernel reads"""
+    res = env["diff_res"]
     Nf = planes[1][..., :3].reshape(-1, 3).astype(np.float64)
     Nr = sr.rotate_hdri(Nf, offset) if offset else Nf
     kd = float(np.float32(1.0) - np.float32(0.04))
     want = kd * sr.sample_cube(env["diff"], res, env["diff_mips"], Nr, 0)[:, :3]
     span = float(env["diff"].max() - env["diff"].min())
     tol = _cube_tol(float(res), 2.0 ** -19, span) + 4 * U24 * np.abs(want).max(1)
-    pf, pv = constants(cam, max_lod, offset)
-    return dict(planes=planes, pf=pf, pv=pv, want=want.reshape(planes[0].shape[:2] + (3,)),
-                tol=tol.reshape(planes[0].shape[:2]))
+    return want.reshape(planes[0].shape[:2] + (3,)), tol.reshape(planes[0].shape[:2])
 
 
 def lut_probe(env, channel, n, seed, max_lod=5):
@@ -195,6 +207,15 @@ def lut_probe(env, channel, n, seed, max_lod=5):
     nrm = np.concatenate([N, r[:, None]], 1)
     alb = np.ones((n, 4), np.float32)
     planes, _ = _frame([pos, nrm, alb])
+    pf, pv = constants(cam, max_lod)
+    want, tol = lut_expect(env, channel, planes, cam)
+    return dict(planes=planes, pf=pf, pv=pv, want=want, tol=tol)
+
+
+def lut_expect(env, channel, planes, cam):
+    """the LUT probe's float64 value and bound, from the G-buffer planes the kernel reads"""
+    lut = env["lut"]
+    H, W = lut.shape[:2]
     V = _v64(planes[0][..., :3].reshape(-1, 3), cam)
     Nf = planes[1][..., :3].reshape(-1, 3).astype(np.float64)
     u = np.clip((Nf * V).sum(1), 0.0, 1.0)
@@ -204,9 +225,7 @@ def lut_probe(env, channel, n, seed, max_lod=5):
     du = 2.0 ** -20 * np.maximum(1.0, np.linalg.norm(Nf, axis=1))
     span = float(lut[..., channel].max() - lut[..., channel].min())
     tol = (W * (du + 2.0 ** -23) + H * 2.0 ** -23) * span + 16 * U24
-    pf, pv = constants(cam, max_lod)
-    return dict(planes=planes, pf=pf, pv=pv, want=np.repeat(want[:, None], 3, 1).reshape(planes[0].shape[:2] + (3,)),
-                tol=tol.reshape(planes[0].shape[:2]))
+    return (np.repeat(want[:, None], 3, 1).reshape(planes[0].shape[:2] + (3,)), tol.reshape(planes[0].shape[:2]))
 
 
 def probe_env(kind, base, channel=0):
