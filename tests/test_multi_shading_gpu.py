@@ -2,8 +2,9 @@
 (vq_forward_lighting_shadowed_multi_signal, vq_forward_lighting_from_materials_multi_signal). Into every destination each call must
 store, bit for bit, what its single-destination call stores into its one output, at rows offset by dst_row_offset, and touch nothing
 else. Simulated worlds (every "rank" on this one GPU, its peers' frames being local destinations) must assemble the frame one
-full-frame call computes, from whole-frame attribute planes with row ranges and from per-rank band planes. No test here starts a
-rendezvous: a signal with n_ranks > 1 needs peers that run at the same time (tools/perf_multi_shading.py under torchrun)."""
+full-frame call computes, from whole-frame attribute planes with row ranges and from per-rank band planes. The tests here pass no
+signal. tests/test_rendezvous_gpu.py runs these calls with one, on one GPU, on flag words whose waits are already satisfied. A
+rendezvous between ranks running at the same time needs two or more GPUs (tools/perf_multi_shading.py under torchrun)."""
 import numpy as np
 import pytest
 import torch
@@ -47,7 +48,9 @@ class Frame:
         rb, re = rows or (0, self.h)
         out = dev(np.full((self.h, self.w, 4), SENTINEL, np.float32))
         c = self.ctx
-        if call == "shadowed":
+        if call == "forward":
+            c.forward_lighting(self.pf, self.pv, self.gbuffer(), self.em, out, row_begin=rb, row_end=re)
+        elif call == "shadowed":
             c.forward_lighting_shadowed(self.pf, self.pv, self.gbuffer(), self.em, out, row_begin=rb, row_end=re, **self.maps)
         elif call == "from_materials":
             c.forward_lighting_from_materials(self.pf, self.pv, self.inputs(), self.table, self.em, out, alpha_mask=self.alpha_mask,
@@ -57,18 +60,22 @@ class Frame:
                                                        alpha_mask=self.alpha_mask, row_begin=rb, row_end=re, **self.maps)
         return host(out)
 
-    def multi(self, call, images, dst_row_offset, rows=None, band=None):
+    def multi(self, call, images, dst_row_offset, rows=None, band=None, signal=None, stream=None):
         """the multi-destination call: rows of the whole-frame inputs, or (band = (a, b)) inputs holding just rows [a, b)"""
         a, b = band or (0, self.h)
         rb, re = rows or (0, b - a)
         c = self.ctx
-        if call == "shadowed":
+        if call == "forward":
+            c.forward_lighting_multi(self.pf, self.pv, self.gbuffer(a, b), self.em, images, dst_row_offset, row_begin=rb, row_end=re,
+                                     signal=signal, stream=stream)
+        elif call == "shadowed":
             c.forward_lighting_shadowed_multi(self.pf, self.pv, self.gbuffer(a, b), self.em, images, dst_row_offset, row_begin=rb,
-                                              row_end=re, **self.maps)
+                                              row_end=re, signal=signal, stream=stream, **self.maps)
         else:
             maps = self.maps if call == "shadowed_from_materials" else {}
             c.forward_lighting_from_materials_multi(self.pf, self.pv, self.inputs(a, b), self.table, self.em, images, dst_row_offset,
-                                                    alpha_mask=self.alpha_mask, row_begin=rb, row_end=re, **maps)
+                                                    alpha_mask=self.alpha_mask, row_begin=rb, row_end=re, signal=signal, stream=stream,
+                                                    **maps)
 
     def world(self, call, n, layout):
         """n simulated ranks, rank r shading its even_tiles band into all n frames (its own first, then the others in rotated

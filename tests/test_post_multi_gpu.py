@@ -2,8 +2,9 @@
 vq_fsr_rcas_multi_signal). Into every destination each call must store, bit for bit, what its single-destination call stores on
 the requested rows, and touch no other row. Simulated worlds (every "rank" on this one GPU, its peers' display frames being local
 destinations) must assemble the display frame the single-GPU chain computes, each rank running its distributed.post_chain_rows
-plan into NaN-filled scratch, so that a row the plan misses would show up as NaN. No test here starts a rendezvous: a signal with
-n_ranks > 1 needs peers that run at the same time (tools/perf_post_multi.py under torchrun)."""
+plan into NaN-filled scratch, so that a row the plan misses would show up as NaN. The tests here pass no signal.
+tests/test_rendezvous_gpu.py runs these calls with one, on one GPU, on flag words whose waits are already satisfied. A rendezvous
+between ranks running at the same time needs two or more GPUs (tools/perf_post_multi.py under torchrun)."""
 import numpy as np
 import pytest
 import torch
@@ -59,17 +60,17 @@ class Pass:
         else:
             c.fsr_rcas(self.con, src, dst)
 
-    def multi(self, src, dsts, rows):
+    def multi(self, src, dsts, rows, signal=None, stream=None):
         imgs = [vq.image_of(d) for d in dsts]
-        c = self.ctx
+        c, kw = self.ctx, dict(signal=signal, stream=stream)
         if self.kind == "tonemap":
-            c.tonemap_multi(self.params, src, imgs, *rows)
+            c.tonemap_multi(self.params, src, imgs, *rows, **kw)
         elif self.kind == "cas":
-            c.cas_multi(self.con, src, imgs, *rows)
+            c.cas_multi(self.con, src, imgs, *rows, **kw)
         elif self.kind == "fsr_easu":
-            c.fsr_easu_multi(self.con, src, imgs, *rows, address_mode=self.mode)
+            c.fsr_easu_multi(self.con, src, imgs, *rows, address_mode=self.mode, **kw)
         else:
-            c.fsr_rcas_multi(self.con, src, imgs, *rows)
+            c.fsr_rcas_multi(self.con, src, imgs, *rows, **kw)
 
 
 def row_ranges(h):
