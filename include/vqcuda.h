@@ -564,6 +564,31 @@ VQ_API int vq_skydome(VqContext* ctx, const VqMatrix* inv_view_proj, VqPyramid h
                       VqImage scene_color, int row_begin, int row_end, void* stream);
 VQ_API int vq_apply_reflections(VqContext* ctx, VqImage scene_color, VqImage reflection_radiance,
                                 const VqImage* bounding_volumes, void* stream);
+/* Both passes on one rank's band of a multi-GPU frame, in the multi-destination form of the vq_*_multi_signal shading calls:
+ * rows [row_begin,row_end) of the per-pixel inputs (normal_mask, reflection_radiance, bounding_volumes: the band only, or the whole
+ * frame) are rows dst_row_offset + y of the frame. outs[0] is the rank's local frame, the source of the band and its first
+ * destination; outs[1..n_outs-1] are the peers' frames mapped into this process. Every destination has the frame's size. One launch,
+ * no context scratch; with a `signal` (n_ranks > 1) the kernel's last CTA runs the rendezvous of VqPeerSignal after every store.
+ *   vq_skydome_multi_signal: afterwards rows dst_row_offset + [row_begin,row_end) of every destination hold, bit for bit, what
+ *     outs[0] holds after vq_skydome on those frame rows with the mask at frame rows: where the mask's xyz is 0 (or everywhere when
+ *     normal_mask is NULL) the sky along the ray through frame pixel (x, dst_row_offset + y); elsewhere what outs[0] already held,
+ *     read back and copied to the peers. So one rank's scene-colour step is its shading call into outs[0] alone (no signal), then
+ *     this call into every rank's frame: each pixel crosses NVLink once and has one writer. Where the alpha mask of a
+ *     from-materials call discarded a pixel, outs[0]'s previous content is what is distributed. For from-materials frames the mask
+ *     is the interpolants' normal_v plane (xyz 0 where nothing was rasterised).
+ *   vq_apply_reflections_multi_signal: vq_apply_reflections in place on the band's rows of outs[0], the result stored into every
+ *     destination. Run it after the sky's rendezvous, when every rank's frame is whole.
+ * Refused with VQ_ERR_INVALID_ARG before the device is touched (also without a context): what the single call refuses; n_outs
+ * outside 1..8, destinations of different sizes, a peer destination equal to outs[0], a negative offset, rows
+ * dst_row_offset + [row_begin,row_end) outside the frame, a signal with n_ranks > 1 and one destination or an empty row range, a
+ * bad signal; a mask, reflection or bounding-volume plane that is not as wide as the frame or has fewer than row_end rows. An empty
+ * row range without a rendezvous launches nothing. */
+VQ_API int vq_skydome_multi_signal(VqContext* ctx, const VqMatrix* inv_view_proj, VqPyramid hdri, const VqImage* normal_mask,
+                                   const VqImage* outs, int n_outs, int dst_row_offset, int row_begin, int row_end,
+                                   const VqPeerSignal* signal, void* stream);
+VQ_API int vq_apply_reflections_multi_signal(VqContext* ctx, VqImage reflection_radiance, const VqImage* bounding_volumes,
+                                             const VqImage* outs, int n_outs, int dst_row_offset, int row_begin, int row_end,
+                                             const VqPeerSignal* signal, void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * SURVEY §8(f).4  Shadowed casters and the hierarchical MIN depth pyramid.

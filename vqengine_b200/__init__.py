@@ -38,6 +38,7 @@ ABI_SYMBOLS = [
     "vq_forward_lighting_shadowed_multi_signal", "vq_forward_lighting_from_materials_multi_signal",
     "vq_tonemap_multi_signal", "vq_cas_multi_signal", "vq_fsr_easu_multi_signal", "vq_fsr_rcas_multi_signal",
     "vq_fsr_easu_source_rows", "vq_post_process", "vq_post_process_multi_signal",
+    "vq_skydome_multi_signal", "vq_apply_reflections_multi_signal",
 ]
 
 
@@ -127,6 +128,10 @@ def _load() -> C.CDLL:
     lib.vq_resize_axis_table.argtypes = [C.c_int, C.c_int, P(C.c_int), P(C.c_int), P(f32), C.c_int, P(C.c_int)]
     lib.vq_skydome.argtypes = [vp, P(Matrix), Pyramid, P(Image), Image, C.c_int, C.c_int, vp]
     lib.vq_apply_reflections.argtypes = [vp, Image, Image, P(Image), vp]
+    lib.vq_skydome_multi_signal.argtypes = [vp, P(Matrix), Pyramid, P(Image), P(Image), C.c_int, C.c_int, C.c_int, C.c_int,
+                                            P(PeerSignal), vp]
+    lib.vq_apply_reflections_multi_signal.argtypes = [vp, Image, P(Image), P(Image), C.c_int, C.c_int, C.c_int, C.c_int,
+                                                      P(PeerSignal), vp]
     lib.vq_forward_lighting_shadowed.argtypes = [vp, P(PerFrameData), P(PerViewLightingData), P(GBuffer), P(EnvironmentMaps),
                                                  P(ShadowMaps), Image, C.c_int, C.c_int, vp]
     lib.vq_forward_lighting_shadowed_from_materials.argtypes = [vp, P(PerFrameData), P(PerViewLightingData), P(SurfaceInputs), vp,
@@ -505,6 +510,29 @@ class Context:
         bv = image_of(bounding_volumes) if bounding_volumes is not None else None
         _check(lib.vq_apply_reflections(self._h, image_of(scene), image_of(reflection),
                                         C.byref(bv) if bv is not None else None, _stream_ptr(stream)))
+
+    # one rank's band of the sky and of the composite into several frames (vq_*_multi_signal): out_images are Image descriptors of
+    # the destinations (the local frame first, then the peers' mapped frames); rows [row_begin, row_end) of the per-pixel inputs are
+    # frame rows dst_row_offset + y (row_end default: the input's height, or the frame rows below the offset without a mask)
+    def skydome_multi(self, inv_view_proj, pyr: Pyramid, out_images, dst_row_offset=0, normal_mask=None, row_begin=0, row_end=None,
+                      stream=None, signal: "PeerSignal" = None):
+        m = Matrix((f32 * 16)(*[float(x) for x in inv_view_proj]))
+        arr = (Image * max(len(out_images), 1))(*out_images)
+        mask = image_of(normal_mask) if normal_mask is not None else None
+        if row_end is None:
+            row_end = mask.height if mask is not None else out_images[0].height - dst_row_offset
+        _check(lib.vq_skydome_multi_signal(self._h, C.byref(m), pyr, C.byref(mask) if mask is not None else None, arr, len(out_images),
+                                           dst_row_offset, row_begin, row_end, C.byref(signal) if signal is not None else None,
+                                           _stream_ptr(stream)))
+
+    def apply_reflections_multi(self, reflection, out_images, dst_row_offset=0, bounding_volumes=None, row_begin=0, row_end=None,
+                                stream=None, signal: "PeerSignal" = None):
+        r = image_of(reflection)
+        bv = image_of(bounding_volumes) if bounding_volumes is not None else None
+        arr = (Image * max(len(out_images), 1))(*out_images)
+        _check(lib.vq_apply_reflections_multi_signal(self._h, r, C.byref(bv) if bv is not None else None, arr, len(out_images),
+                                                     dst_row_offset, row_begin, r.height if row_end is None else row_end,
+                                                     C.byref(signal) if signal is not None else None, _stream_ptr(stream)))
 
     # K11 / K2 / K3 / K4
     def hdri_build_mips(self, pyr: Pyramid, stream=None):

@@ -14,19 +14,12 @@
 using namespace vq;
 
 // =============================================================================================
-// Multi-destination form of K6-K9 (vq_*_multi_signal): the MULTI instantiation of a kernel takes a PostDests where the
-// single-destination one takes its output view. It keeps the full-frame tile grid, launched only over the tile rows that meet
+// Multi-destination form of K6-K9 (vq_*_multi_signal): the MULTI instantiation of a kernel takes a PostDests (vq_common.cuh) where
+// the single-destination one takes its output view. It keeps the full-frame tile grid, launched only over the tile rows that meet
 // [rowBegin, rowEnd) (tile row = blockIdx.y + by0), so every pixel is computed from the same staged values as in the full-frame
 // launch; stores are masked to the range and go to each of the n frames. With a rendezvous (sync.n > 1) the last CTA to retire
-// runs it, as forward_kernel<MULTI> does.
+// runs it (post_retire), as forward_kernel<MULTI> does.
 // =============================================================================================
-struct PostDests {
-    ImgV o[8];
-    int n, w, h;                       // destinations, and the output's size (every destination has it)
-    int rowBegin, rowEnd, by0;
-    PeerSync sync;
-    uint32_t* ticket;                  // retired-CTA count (zero between launches); sync.n > 1 only
-};
 template <bool MULTI> using PostOut = typename std::conditional<MULTI, PostDests, ImgV>::type;
 
 __device__ __forceinline__ unsigned tile_row(const ImgV&) { return blockIdx.y; }
@@ -45,22 +38,6 @@ __device__ __forceinline__ float4* out_row(const ImgV& o, int y) { return o.row(
 __device__ __forceinline__ float4* out_row(const PostDests& d, int y) { return d.o[0].row(y); }
 __device__ __forceinline__ void store_px(const ImgV&, float4* p, int, int, float4 v) { st_stream(p, v); }
 __device__ __forceinline__ void store_px(const PostDests& d, float4*, int x, int y, float4 v) { store_px(d, x, y, v); }
-// Every thread of the CTA calls it once: after its last store, or where it leaves early. The barrier is the non-aligned
-// barrier.sync, which threads may reach from different places in the kernel.
-__device__ __forceinline__ void post_retire(const ImgV&) {}
-__device__ __forceinline__ void post_retire(const PostDests& d) {
-    if (d.sync.n <= 1) return;
-    __threadfence_system();            // this thread's peer stores are ordered before the CTA's retirement
-    asm volatile("barrier.sync 0;" ::: "memory");
-    if (threadIdx.x == 0 && threadIdx.y == 0) {
-        const uint32_t done = atomicAdd(d.ticket, 1u);
-        if (done == gridDim.x * gridDim.y - 1u) {
-            *d.ticket = 0u;
-            __threadfence_system();
-            peer_rendezvous(d.sync);
-        }
-    }
-}
 
 // =============================================================================================
 // K6 Tonemapper — Shaders/Tonemapper.hlsl:110-151, Shaders/HDR.hlsl:76-119
