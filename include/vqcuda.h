@@ -9,10 +9,20 @@
  *     described by {ptr, width, height, pitch}); the library never frees caller memory;
  *   - nothing throws across the boundary: every call returns 0 (VQ_OK) or a negative
  *     VqStatus; vq_last_error() gives a thread-local message;
- *   - calls only ENQUEUE work on `stream` (== recording into a command list); they are
- *     thread-safe when callers use distinct streams (== per-thread command lists,
- *     SceneRendering.cpp:197-207): host-side context state is guarded by a lock and every
- *     SPD launch gets its own ticket word. EXCEPTIONS — calls whose DEVICE scratch is one
+ *   - calls that take `stream` only ENQUEUE work on it (== recording into a command list):
+ *     they return without waiting for earlier work on `stream`, their kernels and copies
+ *     read the inputs and write the outputs after that work, and nothing runs on another
+ *     stream. One exception: a call that has to GROW context scratch (the first call at a
+ *     larger size: the environment sampling copies of an unregistered environment, the PCF
+ *     records of vq_forward_lighting_shadowed*, vq_image_resize's intermediate and tables,
+ *     vq_depth_min_pyramid's pads, and vq_ctx_resize's host-call staging) first waits for
+ *     the whole device (cudaDeviceSynchronize: an earlier launch on any stream may still
+ *     read the old buffer), then enqueues. Pre-size with a first call at the largest size
+ *     (or vq_ctx_resize) so that steady frames never wait;
+ *   - they are thread-safe when callers use distinct streams (== per-thread command lists,
+ *     SceneRendering.cpp:197-207): host-side context state is guarded by a lock, the error
+ *     message is per thread, and every SPD or persistent launch takes its own ticket word
+ *     from a ring of 128 (see below). EXCEPTIONS — calls whose DEVICE scratch is one
  *     buffer per context and which therefore must not be in flight concurrently on two
  *     streams of the same context (use one context per thread for these, or order them):
  *       vq_forward_lighting* with an environment that is NOT registered by
@@ -20,8 +30,18 @@
  *       vq_environment_prepare itself, vq_image_resize, vq_depth_min_pyramid,
  *       vq_forward_lighting_shadowed and vq_forward_lighting_shadowed_multi_signal (per-pixel PCF records),
  *       vq_forward_lighting_host.
+ *     Ticket ring: the SPD kernels (vq_spd_downsample, vq_hdri_build_mips up to 4096^2) and
+ *     the persistent or signalled kernels (K3, and every *_multi_signal / *_ranges call with
+ *     a signal of n_ranks > 1) take words from one counter per context, 256 single words
+ *     and 128 word pairs. Two launches running at the same time share a word if at least
+ *     128 such calls on the context were made between them (e.g. a long prefilter on one
+ *     stream while 128 SPD or K3 calls are issued on another): keep fewer in flight.
  *     Synchronisation is the caller's (cudaStreamSynchronize == fence wait), except the
- *     *_host convenience calls which block.
+ *     blocking calls below;
+ *   - the BLOCKING calls (vq_forward_lighting_host, vq_hdr_load_host, vq_hdr_save_host,
+ *     vq_material_table_create) wait for the whole device first, so they are ordered after
+ *     all device work enqueued before them on ANY stream (legacy, blocking or non-blocking),
+ *     and return with their own work complete. They do not wait for work enqueued later.
  *   - there is NO CPU fallback: without a CUDA device every device call fails with
  *     VQ_ERR_NO_DEVICE.
  *
@@ -515,7 +535,8 @@ VQ_API int vq_hdr_parse(const void* file, uint64_t size, VqHdrInfo* info, uint64
  * dev_max_luminance (optional): receives max over texels of 0.2126 r + 0.7152 g + 0.0722 b (Image::MaxLuminance). */
 VQ_API int vq_hdr_decode(VqContext* ctx, const void* dev_file, uint64_t size, const VqHdrInfo* info,
                          const uint64_t* dev_channel_offsets, VqImage out, float* dev_max_luminance, void* stream);
-/* Blocking: host file image -> device fp32 image (parse + upload + decode). */
+/* Blocking: host file image -> device fp32 image (parse + upload + decode). Ordered after all earlier device work, on any
+ * stream (the header's blocking calls): a kernel still reading `out` finishes before it is overwritten. */
 VQ_API int vq_hdr_load_host(VqContext* ctx, const void* host_file, uint64_t size, VqImage out, float* max_luminance);
 /* DEVICE. RGBA32F -> RGBE texels (4 bytes each, tightly packed rows), stbiw__linear_to_rgbe, for every float input:
  *   maxcomp = max(r, max(g, b)) with max(a, b) = a > b ? a : b, stb's nesting: a NaN in r or g is ignored
@@ -529,7 +550,8 @@ VQ_API int vq_hdr_load_host(VqContext* ctx, const void* host_file, uint64_t size
 VQ_API int vq_hdr_encode_rgbe(VqContext* ctx, VqImage in, void* dev_rgbe, void* stream);
 /* HOST. RGBE texels -> the .hdr file image (text header + per-scanline run lists). file == NULL: size query. */
 VQ_API int vq_hdr_pack_file(const void* host_rgbe, int width, int height, void* file, uint64_t capacity, uint64_t* size);
-/* Blocking: device fp32 image -> host file image (encode + download + pack). */
+/* Blocking: device fp32 image -> host file image (encode + download + pack). Ordered after all earlier device work, on any
+ * stream: a kernel still writing `in` finishes before it is encoded. */
 VQ_API int vq_hdr_save_host(VqContext* ctx, VqImage in, void* host_file, uint64_t capacity, uint64_t* size);
 
 /* Image::CreateResizedImage (Image.cpp:148-190) -> stbir_resize_float(in, w, h, 0, out, W, H, 0, 4): the downsize the engine

@@ -38,6 +38,9 @@ extern "C" int vq_forward_lighting_host(VqContext* ctx, const VqPerFrameData* pf
         VQ_REQUIRE(im->width == W && im->height == H, "every host G-buffer plane must have the output's width and height");
     if (hasEm) VQ_REQUIRE(vq_image_ok(hgb->emissive) && hgb->emissive.width == W && hgb->emissive.height == H,
                           "bad host emissive plane (descriptor, pitch or size)");
+    // blocking: ordered after all device work enqueued before the call, on any stream (the pipeline's own streams are
+    // non-blocking and would not wait for the caller's work on the environment maps)
+    VQ_CUDA_OK(cudaDeviceSynchronize());
     const int planes = hasEm ? 5 : 4;
     const size_t rowBytes = (size_t)W * 16, planeBytes = rowBytes * H;
     VqScratchLock lock(ctx);           // the staging buffer, the three streams and the event ring are the context's

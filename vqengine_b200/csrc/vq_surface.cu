@@ -201,14 +201,15 @@ extern "C" int vq_material_table_create(VqContext* ctx, const VqMaterialData* ma
     }
     VqMaterialTable* t = (VqMaterialTable*)calloc(1, sizeof(VqMaterialTable));
     if (!t) { free(host); free(recOffset); free(recCount); vq_set_error("out of host memory"); return VQ_ERR_OUT_OF_MEMORY; }
-    cudaError_t e = cudaSuccess;
-    if (recTexels) {
+    // blocking: ordered after all device work enqueued before the call, on any stream (mip chains may still be in flight on the
+    // caller's streams, and the sampling copies below read them)
+    cudaError_t e = cudaDeviceSynchronize();
+    if (e == cudaSuccess && recTexels) {
         // a sampling copy is an optimisation: when it does not fit, the materials simply stay on the map-by-map path
         if (cudaMalloc(&t->records, (size_t)recTexels * 16) != cudaSuccess) { cudaGetLastError(); t->records = nullptr; recTexels = 0; }
         else t->record_bytes = (size_t)recTexels * 16;
     }
-    if (t->records) {
-        e = cudaDeviceSynchronize();                                    // mip chains may still be in flight on the caller's streams
+    if (e == cudaSuccess && t->records) {
         for (int i = 0; e == cudaSuccess && i < count; ++i) {
             if (!recCount[i]) continue;
             const VqTexture2D* src = &textures[i].diffuse;
