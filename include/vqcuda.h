@@ -256,6 +256,7 @@ typedef struct VqDiffuseIrradianceParams {
 VQ_API int vq_diffuse_irradiance(VqContext* ctx, const VqDiffuseIrradianceParams* params,
                                  VqPyramid hdri, VqCubemap out,
                                  int row_begin, int row_end, void* stream);
+/* One rank's band of K2 into every rank's cube: vq_diffuse_irradiance_multi_signal (vqcuda_prefilter_multi.h). */
 
 /* ------------------------------------------------------------------------------------------
  * K3  Specular prefilter (GGX importance sampling, 512 Hammersley samples, PDF-based source mip).
@@ -289,6 +290,7 @@ VQ_API int vq_specular_prefilter_ranges(VqContext* ctx, VqPyramid hdri, const Vq
  * ------------------------------------------------------------------------------------------ */
 VQ_API int vq_brdf_integration_lut(VqContext* ctx, VqImage out_rg, int num_samples,
                                    int row_begin, int row_end, void* stream);
+/* One rank's band of K4 into every rank's LUT: vq_brdf_integration_lut_multi_signal (vqcuda_prefilter_multi.h). */
 
 /* ------------------------------------------------------------------------------------------
  * K5  Separable 21-tap Gaussian blur, clamp-to-edge, alpha = 1.  Replaces the dispatches at
@@ -297,6 +299,7 @@ VQ_API int vq_brdf_integration_lut(VqContext* ctx, VqImage out_rg, int num_sampl
  * ------------------------------------------------------------------------------------------ */
 VQ_API int vq_gaussian_blur_x(VqContext* ctx, const VqBlurParams* params, VqImage in, VqImage out, void* stream);
 VQ_API int vq_gaussian_blur_y(VqContext* ctx, const VqBlurParams* params, VqImage in, VqImage out, void* stream);
+/* A whole one-mip cube, X then Y, in one launch: vq_gaussian_blur_cube (vqcuda_prefilter_multi.h). */
 
 /* ------------------------------------------------------------------------------------------
  * K6  Tonemapper.  Replaces the dispatch at SceneRendering.cpp:2640-2656 + CSMain (Tonemapper.hlsl:110-151).
@@ -685,4 +688,8 @@ VQ_API int vq_forward_lighting_host(VqContext* ctx,
 #ifdef __cplusplus
 }
 #endif
+
+/* The environment prefilter across GPUs: the band forms of K2 and K4 and the one-launch cube blur. */
+#include "vqcuda_prefilter_multi.h"
+
 #endif /* VQCUDA_H */

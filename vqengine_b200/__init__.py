@@ -40,6 +40,8 @@ ABI_SYMBOLS = [
     "vq_fsr_easu_source_rows", "vq_post_process", "vq_post_process_multi_signal",
     "vq_skydome_multi_signal", "vq_apply_reflections_multi_signal",
 ]
+# every symbol include/vqcuda_prefilter_multi.h declares (the environment prefilter across GPUs; vqcuda.h includes that header)
+PREFILTER_MULTI_SYMBOLS = ["vq_diffuse_irradiance_multi_signal", "vq_brdf_integration_lut_multi_signal", "vq_gaussian_blur_cube"]
 
 
 class VqError(RuntimeError):
@@ -78,6 +80,10 @@ def _load() -> C.CDLL:
     lib.vq_specular_prefilter_multi.argtypes = [vp, Pyramid, P(Cubemap), C.c_int, C.c_int, C.c_int, C.c_int, vp]
     lib.vq_specular_prefilter_ranges.argtypes = [vp, Pyramid, P(Cubemap), C.c_int, C.c_int, P(C.c_int), C.c_int, P(PeerSignal), vp]
     lib.vq_brdf_integration_lut.argtypes = [vp, Image, C.c_int, C.c_int, C.c_int, vp]
+    lib.vq_diffuse_irradiance_multi_signal.argtypes = [vp, P(DiffuseIrradianceParams), Pyramid, P(Cubemap), C.c_int, C.c_int, C.c_int,
+                                                       P(PeerSignal), vp]
+    lib.vq_brdf_integration_lut_multi_signal.argtypes = [vp, P(Image), C.c_int, C.c_int, C.c_int, C.c_int, P(PeerSignal), vp]
+    lib.vq_gaussian_blur_cube.argtypes = [vp, Cubemap, Cubemap, vp]
     lib.vq_gaussian_blur_x.argtypes = [vp, P(BlurParams), Image, Image, vp]
     lib.vq_gaussian_blur_y.argtypes = [vp, P(BlurParams), Image, Image, vp]
     lib.vq_tonemap.argtypes = [vp, P(TonemapperParams), Image, Image, vp]
@@ -544,6 +550,16 @@ class Context:
         _check(lib.vq_diffuse_irradiance(self._h, C.byref(p), pyr, cube, row_begin,
                                          6 * cube.res if row_end is None else row_end, _stream_ptr(stream)))
 
+    def diffuse_irradiance_multi(self, pyr: Pyramid, cubes, step=0.0, n_phi=64, n_theta=16, src_mip=3, row_begin=0, row_end=None,
+                                 stream=None, signal: "PeerSignal" = None):
+        """diffuse_irradiance on rows [row_begin, row_end) into every cube of `cubes` (Cubemap descriptors of one shape, the local
+        cube first, then the peers' mapped cubes); signal: the in-kernel cross-rank rendezvous"""
+        p = DiffuseIrradianceParams(step, n_phi, n_theta, src_mip)
+        arr = (Cubemap * max(len(cubes), 1))(*cubes)
+        _check(lib.vq_diffuse_irradiance_multi_signal(self._h, C.byref(p), pyr, arr, len(cubes), row_begin,
+                                                      6 * cubes[0].res if row_end is None else row_end,
+                                                      C.byref(signal) if signal is not None else None, _stream_ptr(stream)))
+
     def specular_prefilter(self, pyr: Pyramid, cube: Cubemap, num_samples=512, row_begin=0, row_end=None, stream=None):
         _check(lib.vq_specular_prefilter(self._h, pyr, cube, num_samples, row_begin,
                                          cubemap_row_count(cube.res, cube.mips) if row_end is None else row_end,
@@ -568,6 +584,19 @@ class Context:
         o = image_of(out, 2)
         _check(lib.vq_brdf_integration_lut(self._h, o, num_samples, row_begin,
                                            o.height if row_end is None else row_end, _stream_ptr(stream)))
+
+    def brdf_integration_lut_multi(self, out_images, num_samples=2048, row_begin=0, row_end=None, stream=None,
+                                   signal: "PeerSignal" = None):
+        """brdf_integration_lut on rows [row_begin, row_end) into every LUT of `out_images` (float2 Image descriptors of one size,
+        the local LUT first); signal: the in-kernel cross-rank rendezvous"""
+        arr = (Image * max(len(out_images), 1))(*out_images)
+        _check(lib.vq_brdf_integration_lut_multi_signal(self._h, arr, len(out_images), num_samples, row_begin,
+                                                        out_images[0].height if row_end is None else row_end,
+                                                        C.byref(signal) if signal is not None else None, _stream_ptr(stream)))
+
+    def gaussian_blur_cube(self, src: Cubemap, dst: Cubemap, stream=None):
+        """every face of a one-mip cube blurred X then Y in one launch (src may be dst)"""
+        _check(lib.vq_gaussian_blur_cube(self._h, src, dst, _stream_ptr(stream)))
 
     # post chain
     def gaussian_blur(self, src, dst, vertical: bool, stream=None):

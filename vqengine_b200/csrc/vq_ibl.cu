@@ -49,9 +49,19 @@ struct DiffuseArgs {
     PyrV hdri; float4* out; int res; int rowBegin; int texels;   // texels = rows * res
     float step; int nPhi, nTheta; int srcMip;
 };
+// The multi-destination form (vq_diffuse_irradiance_multi_signal): every texel goes to each of n packed cubemaps (the local one
+// first, then the peers'), and the last CTA to retire runs the rendezvous (cta_retire). A.out is unused.
+struct DiffuseMultiArgs {
+    DiffuseArgs a;
+    float4* o[8]; int n;
+    PeerSync sync;
+    uint32_t* ticket;                    // retired-CTA count (zero between launches); sync.n > 1 only
+};
 
-__global__ void __launch_bounds__(IBL_THREADS) diffuse_irradiance_kernel(const __grid_constant__ DiffuseArgs A) {
-    extern __shared__ float smem[];
+// The texels of K2 that this CTA's warps own, each handed to store(texel index, value) by lane 0 of its warp. A texel's bits depend
+// only on its own warp (lane-strided sums, then the warp_sum butterfly), not on the CTA or the grid it runs in.
+template <class Store>
+__device__ __forceinline__ void diffuse_texels(const DiffuseArgs& A, float* smem, Store store) {
     float* sSinP = smem;                 // [nPhi]
     float* sCosP = sSinP + A.nPhi;       // [nPhi]
     float* sSinT = sCosP + A.nPhi;       // [nTheta]
@@ -96,9 +106,24 @@ __global__ void __launch_bounds__(IBL_THREADS) diffuse_irradiance_kernel(const _
         acc.x = warp_sum(acc.x); acc.y = warp_sum(acc.y); acc.z = warp_sum(acc.z);
         if (lane == 0) {
             const float n = (float)nSamples;     // numSamples += 1.0f per sample: exact below 2^24
-            A.out[(size_t)fr * A.res + px] = make_float4(PI * acc.x / n, PI * acc.y / n, PI * acc.z / n, 1.0f);
+            store((size_t)fr * A.res + px, make_float4(PI * acc.x / n, PI * acc.y / n, PI * acc.z / n, 1.0f));
         }
     }
+}
+
+__global__ void __launch_bounds__(IBL_THREADS) diffuse_irradiance_kernel(const __grid_constant__ DiffuseArgs A) {
+    extern __shared__ float smem[];
+    diffuse_texels(A, smem, [&](size_t i, float4 o) { A.out[i] = o; });
+}
+
+__global__ void __launch_bounds__(IBL_THREADS) diffuse_irradiance_multi_kernel(const __grid_constant__ DiffuseMultiArgs M) {
+    extern __shared__ float smem[];
+    diffuse_texels(M.a, smem, [&](size_t i, float4 o) {
+#pragma unroll
+        for (int q = 0; q < 8; ++q)      // constant indices: the pointers stay in the parameter bank
+            if (q < M.n) M.o[q][i] = o;
+    });
+    cta_retire(M);
 }
 
 // =============================================================================================
@@ -258,9 +283,18 @@ __global__ void __launch_bounds__(IBL_THREADS) specular_persistent_kernel(const 
 // K4 BRDF integration LUT
 // =============================================================================================
 struct LutArgs { float2* out; int w, h, pitch2; int rowBegin; int numSamples; };
+// The multi-destination form (vq_brdf_integration_lut_multi_signal): n float2 images of one size (the local one first, then the
+// peers'), each with its own pitch; the last CTA to retire runs the rendezvous. A.out and A.pitch2 are unused.
+struct LutMultiArgs {
+    LutArgs a;
+    float2* o[8]; int pitch2[8]; int n;
+    PeerSync sync;
+    uint32_t* ticket;                    // retired-CTA count (zero between launches); sync.n > 1 only
+};
 
-__global__ void __launch_bounds__(256) brdf_lut_kernel(const __grid_constant__ LutArgs A) {
-    extern __shared__ float4 sHw[];      // world-space half vectors for this row's roughness (N = +Z)
+// One CTA: texels [256 blockIdx.x, +256) of row rowBegin + blockIdx.y, each handed to store(x, y, value) by its thread
+template <class Store>
+__device__ __forceinline__ void brdf_lut_texels(const LutArgs& A, float4* sHw, Store store) {
     const int y = A.rowBegin + blockIdx.y;
     const float roughness = ((float)y + 0.5f) / (float)A.h;                  // CubemapConvolution.hlsl:234-236
     for (int i = threadIdx.x; i < A.numSamples; i += 256) {
@@ -304,7 +338,22 @@ __global__ void __launch_bounds__(256) brdf_lut_kernel(const __grid_constant__ L
         }
     }
     const float n = (float)A.numSamples;
-    A.out[(size_t)y * A.pitch2 + x] = make_float2(F0Scale / n, F0Bias / n);
+    store(x, y, make_float2(F0Scale / n, F0Bias / n));
+}
+
+__global__ void __launch_bounds__(256) brdf_lut_kernel(const __grid_constant__ LutArgs A) {
+    extern __shared__ float4 sHw[];      // world-space half vectors for this row's roughness (N = +Z)
+    brdf_lut_texels(A, sHw, [&](int x, int y, float2 v) { A.out[(size_t)y * A.pitch2 + x] = v; });
+}
+
+__global__ void __launch_bounds__(256) brdf_lut_multi_kernel(const __grid_constant__ LutMultiArgs M) {
+    extern __shared__ float4 sHw[];
+    brdf_lut_texels(M.a, sHw, [&](int x, int y, float2 v) {
+#pragma unroll
+        for (int q = 0; q < 8; ++q)
+            if (q < M.n) M.o[q][(size_t)y * M.pitch2[q] + x] = v;
+    });
+    cta_retire(M);        // also the threads past the row's last texel, which left brdf_lut_texels early
 }
 
 }  // namespace
@@ -331,10 +380,9 @@ extern "C" int vq_hdri_build_mips(VqContext* ctx, VqPyramid hd, void* stream) {
     return VQ_OK;
 }
 
-extern "C" int vq_diffuse_irradiance(VqContext* ctx, const VqDiffuseIrradianceParams* p, VqPyramid hd, VqCubemap out,
-                                     int row_begin, int row_end, void* stream) {
-    int rc = vq_enter(ctx); if (rc) return rc;
-    VQ_MARK("DiffuseIrradianceCubemap");
+// K2's argument checks and launch parameters (every field of A but A.out), shared by the single and the multi-destination call
+static int diffuse_setup(const VqDiffuseIrradianceParams* p, VqPyramid hd, VqCubemap out, int row_begin, int row_end,
+                         DiffuseArgs& A, size_t& smem) {
     VQ_REQUIRE(p, "params is null");
     VQ_REQUIRE(pyr_ok(hd), "bad HDRI pyramid descriptor");
     VQ_REQUIRE(out.ptr && out.res >= 2 && out.mips == 1, "diffuse irradiance cubemap must have 1 mip");
@@ -348,19 +396,62 @@ extern "C" int vq_diffuse_irradiance(VqContext* ctx, const VqDiffuseIrradiancePa
         nTheta = 0; for (float th = 0.0f; th < 1.5707963268f; th += p->step) { if (++nTheta > (1 << 20)) break; }
     } else { nPhi = p->n_phi; nTheta = p->n_theta; }
     VQ_REQUIRE(nPhi >= 1 && nTheta >= 1 && (long long)nPhi * nTheta < (1 << 24), "sample grid out of range");
-    const size_t smem = (size_t)(2 * nPhi + 2 * nTheta) * sizeof(float);
+    smem = (size_t)(2 * nPhi + 2 * nTheta) * sizeof(float);
     VQ_REQUIRE(smem <= 200 * 1024, "sample grid does not fit shared memory");
-    if (row_begin == row_end) return VQ_OK;
-    DiffuseArgs A;
-    A.hdri = make_pyr(hd); A.out = (float4*)out.ptr; A.res = out.res; A.rowBegin = row_begin;
+    A.hdri = make_pyr(hd); A.out = nullptr; A.res = out.res; A.rowBegin = row_begin;
     A.texels = (row_end - row_begin) * out.res;
     A.step = p->step > 0.0f ? p->step : 0.0f; A.nPhi = nPhi; A.nTheta = nTheta; A.srcMip = p->src_mip;
-    if (smem > 48 * 1024) VQ_CUDA_OK(cudaFuncSetAttribute(diffuse_irradiance_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    int blocks = (A.texels + IBL_WARPS - 1) / IBL_WARPS;
+    return VQ_OK;
+}
+
+// K2's grid: one warp per texel, at most 8 CTAs per SM (the CTAs stride over the texels)
+static int diffuse_blocks(const VqContext* ctx, int texels) {
+    int blocks = (texels + IBL_WARPS - 1) / IBL_WARPS;
     const int cap = ctx->sm_count * 8;
-    if (blocks > cap) blocks = cap;
-    diffuse_irradiance_kernel<<<blocks, IBL_THREADS, smem, (cudaStream_t)stream>>>(A);
+    return blocks > cap ? cap : blocks;
+}
+
+extern "C" int vq_diffuse_irradiance(VqContext* ctx, const VqDiffuseIrradianceParams* p, VqPyramid hd, VqCubemap out,
+                                     int row_begin, int row_end, void* stream) {
+    int rc = vq_enter(ctx); if (rc) return rc;
+    VQ_MARK("DiffuseIrradianceCubemap");
+    DiffuseArgs A;
+    size_t smem = 0;
+    rc = diffuse_setup(p, hd, out, row_begin, row_end, A, smem); if (rc) return rc;
+    if (row_begin == row_end) return VQ_OK;
+    A.out = (float4*)out.ptr;
+    if (smem > 48 * 1024) VQ_CUDA_OK(cudaFuncSetAttribute(diffuse_irradiance_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    diffuse_irradiance_kernel<<<diffuse_blocks(ctx, A.texels), IBL_THREADS, smem, (cudaStream_t)stream>>>(A);
     return vq_check_launch("diffuse_irradiance");
+}
+
+// K2 on rows [row_begin, row_end) into every destination cubemap (one rank's band of a multi-GPU prefilter), with the optional
+// in-kernel rendezvous. Every argument is checked before the device is touched.
+extern "C" int vq_diffuse_irradiance_multi_signal(VqContext* ctx, const VqDiffuseIrradianceParams* p, VqPyramid hd,
+                                                  const VqCubemap* outs, int n_outs, int row_begin, int row_end,
+                                                  const VqPeerSignal* signal, void* stream) {
+    VQ_REQUIRE(outs, "null destination list");
+    VQ_REQUIRE(n_outs >= 1 && n_outs <= 8, "1..8 destinations");
+    DiffuseMultiArgs M;
+    memset(&M, 0, sizeof(M));
+    size_t smem = 0;
+    int rc = diffuse_setup(p, hd, outs[0], row_begin, row_end, M.a, smem); if (rc) return rc;
+    for (int k = 1; k < n_outs; ++k) {
+        VQ_REQUIRE(outs[k].ptr && outs[k].res == outs[0].res && outs[k].mips == outs[0].mips, "every destination cubemap must have the same shape");
+        VQ_REQUIRE(outs[k].ptr != outs[0].ptr, "a peer destination must not be the local cubemap outs[0]");
+    }
+    VQ_REQUIRE(row_begin < row_end || !(signal && signal->n_ranks > 1), "a rendezvous needs a non-empty row range (the kernel runs it)");
+    rc = vq_fill_peer_sync(signal, &M.sync); if (rc) return rc;
+    VQ_REQUIRE(M.sync.n == 0 || n_outs > 1, "a rendezvous only makes sense with peer destinations");
+    rc = vq_enter(ctx); if (rc) return rc;
+    VQ_MARK("DiffuseIrradianceCubemap");
+    if (row_begin == row_end) return VQ_OK;
+    for (int k = 0; k < n_outs; ++k) M.o[k] = (float4*)outs[k].ptr;
+    M.n = n_outs;
+    M.ticket = M.sync.n > 1 ? vq_ticket_pair(ctx) : nullptr;
+    if (smem > 48 * 1024) VQ_CUDA_OK(cudaFuncSetAttribute(diffuse_irradiance_multi_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    diffuse_irradiance_multi_kernel<<<diffuse_blocks(ctx, M.a.texels), IBL_THREADS, smem, (cudaStream_t)stream>>>(M);
+    return vq_check_launch("diffuse_irradiance_multi");
 }
 
 // ranges: n_ranges pairs [begin,end) of the flattened (mip, face, row) space, in increasing order and disjoint
@@ -469,4 +560,36 @@ extern "C" int vq_brdf_integration_lut(VqContext* ctx, VqImage out, int num_samp
     const dim3 grid((out.width + 255) / 256, row_end - row_begin);
     brdf_lut_kernel<<<grid, 256, smem, (cudaStream_t)stream>>>(A);
     return vq_check_launch("brdf_integration_lut");
+}
+
+// K4 on rows [row_begin, row_end) into every destination LUT (one rank's band), with the optional in-kernel rendezvous. Every
+// argument is checked before the device is touched.
+extern "C" int vq_brdf_integration_lut_multi_signal(VqContext* ctx, const VqImage* outs, int n_outs, int num_samples, int row_begin,
+                                                    int row_end, const VqPeerSignal* signal, void* stream) {
+    VQ_REQUIRE(outs, "null destination list");
+    VQ_REQUIRE(n_outs >= 1 && n_outs <= 8, "1..8 destinations");
+    for (int k = 0; k < n_outs; ++k) {
+        VQ_REQUIRE(vq_image_ok(outs[k], 8), "bad LUT image descriptor (float2 texels)");
+        VQ_REQUIRE(outs[k].width == outs[0].width && outs[k].height == outs[0].height, "every destination must have the size of the first");
+        VQ_REQUIRE(k == 0 || outs[k].ptr != outs[0].ptr, "a peer destination must not be the local LUT outs[0]");
+    }
+    VQ_REQUIRE(num_samples >= 1 && num_samples <= 8192, "num_samples out of range");
+    VQ_REQUIRE(row_begin >= 0 && row_end <= outs[0].height && row_begin <= row_end, "row range out of bounds");
+    VQ_REQUIRE(row_begin < row_end || !(signal && signal->n_ranks > 1), "a rendezvous needs a non-empty row range (the kernel runs it)");
+    LutMultiArgs M;
+    memset(&M, 0, sizeof(M));
+    int rc = vq_fill_peer_sync(signal, &M.sync); if (rc) return rc;
+    VQ_REQUIRE(M.sync.n == 0 || n_outs > 1, "a rendezvous only makes sense with peer destinations");
+    rc = vq_enter(ctx); if (rc) return rc;
+    VQ_MARK("CreateBRDFIntegralLUT");
+    if (row_begin == row_end) return VQ_OK;
+    M.a.w = outs[0].width; M.a.h = outs[0].height; M.a.rowBegin = row_begin; M.a.numSamples = num_samples;
+    for (int k = 0; k < n_outs; ++k) { M.o[k] = (float2*)outs[k].ptr; M.pitch2[k] = (int)(outs[k].pitch_bytes / 8); }
+    M.n = n_outs;
+    M.ticket = M.sync.n > 1 ? vq_ticket_pair(ctx) : nullptr;
+    const size_t smem = (size_t)num_samples * sizeof(float4);
+    if (smem > 48 * 1024) VQ_CUDA_OK(cudaFuncSetAttribute(brdf_lut_multi_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    const dim3 grid((outs[0].width + 255) / 256, row_end - row_begin);
+    brdf_lut_multi_kernel<<<grid, 256, smem, (cudaStream_t)stream>>>(M);
+    return vq_check_launch("brdf_integration_lut_multi");
 }

@@ -140,6 +140,30 @@ extern "C" int vq_tonemap(VqContext* ctx, const VqTonemapperParams* p, VqImage i
 __constant__ float c_gauss[11] = {0.224716f, 0.191756f, 0.119146f, 0.053897f, 0.017746f, 0.004252f,
                                   0.000741f, 0.000094f, 0.000009f, 0.000001f, 0.0f};   // GaussianBlur.hlsl:110
 
+// The per-pixel tap sums, shared by every blur kernel: tap(k), k = 0..20, is the (clamped) sample at offset k - 10 along the pass's
+// axis; the products are accumulated with fmaf in the HLSL loop's kernelIt order 0..20, so every kernel rounds alike.
+template <class Tap>
+__device__ __forceinline__ float gauss21(Tap tap) {
+    float a = 0.0f;
+#pragma unroll
+    for (int k = 0; k < 21; ++k) {                                       // kernelIt order 0..20 as in the HLSL loop
+        const int ki = k < 10 ? 10 - k : k - 10;
+        a = fmaf(tap(k), c_gauss[ki], a);
+    }
+    return a;
+}
+template <class Tap>
+__device__ __forceinline__ float3 gauss21_3(Tap tap) {                  // the three colour channels, each as gauss21
+    float3 a = f3(0.0f);
+#pragma unroll
+    for (int k = 0; k < 21; ++k) {
+        const float w = c_gauss[k < 10 ? 10 - k : k - 10];
+        const float3 v = tap(k);
+        a.x = fmaf(v.x, w, a.x); a.y = fmaf(v.y, w, a.y); a.z = fmaf(v.z, w, a.z);
+    }
+    return a;
+}
+
 // X pass: a CTA owns a 512-pixel column strip and walks BX_XR consecutive rows. Each row's BX_W+24 pixels are staged into
 // PLANAR shared memory (R,G,B planes) so that each thread reads its 28-value window with conflict-free LDS.128 and
 // produces 4 adjacent pixels from registers (sliding window: 7 LDS.128 per channel per 4 pixels). The next row's global
@@ -191,15 +215,8 @@ __global__ void __launch_bounds__(BX_T) blur_x_kernel(ImgV in, ImgV out, int siz
 #pragma unroll
             for (int q = 0; q < 7; ++q) { const float4 v = p[q]; win[4 * q] = v.x; win[4 * q + 1] = v.y; win[4 * q + 2] = v.z; win[4 * q + 3] = v.w; }
 #pragma unroll
-            for (int j = 0; j < 4; ++j) {
-                float a = 0.0f;
-#pragma unroll
-                for (int k = 0; k < 21; ++k) {                           // kernelIt order 0..20 as in the HLSL loop
-                    const int ki = k < 10 ? 10 - k : k - 10;
-                    a = fmaf(win[j + 2 + k], c_gauss[ki], a);            // tap at x+j-10+k -> window index j+2+k
-                }
-                acc[c][j] = a;
-            }
+            for (int j = 0; j < 4; ++j)                                  // tap at x+j-10+k -> window index j+2+k
+                acc[c][j] = gauss21([&](int k) { return win[j + 2 + k]; });
         }
 #pragma unroll
         for (int j = 0; j < 4; ++j) so[warp][lane * 4 + j] = make_float4(acc[0][j], acc[1][j], acc[2][j], 1.0f);
@@ -245,13 +262,7 @@ __global__ void __launch_bounds__(BYM_T) blur_y_kernel(ImgV in, ImgV out, int si
             // newest row y+10 (requested BYM_PRE iterations ago) goes to slot (20+u)%21; request row y+10+BYM_PRE
             ring[(20 + u) % 21] = pre[u % BYM_PRE];
             pre[u % BYM_PRE] = xyz(__ldg(src + (size_t)min(y + 10 + BYM_PRE, sizeY - 1) * pin));
-            float3 a = f3(0.0f);
-#pragma unroll
-            for (int k = 0; k < 21; ++k) {                           // kernelIt order 0..20 as in the HLSL loop
-                const float w = c_gauss[k < 10 ? 10 - k : k - 10];
-                const float3 v = ring[(u + k) % 21];
-                a.x = fmaf(v.x, w, a.x); a.y = fmaf(v.y, w, a.y); a.z = fmaf(v.z, w, a.z);
-            }
+            const float3 a = gauss21_3([&](int k) { return ring[(u + k) % 21]; });
             if (y < sizeY) st_stream(dst + (size_t)y * pout, make_float4(a.x, a.y, a.z, 1.0f));
         }
     }
@@ -278,6 +289,54 @@ static int blur_common(VqContext* ctx, const VqBlurParams* p, VqImage in, VqImag
 }
 extern "C" int vq_gaussian_blur_x(VqContext* ctx, const VqBlurParams* p, VqImage in, VqImage out, void* stream) { VQ_MARK("BlurX"); return blur_common(ctx, p, in, out, stream, false); }
 extern "C" int vq_gaussian_blur_y(VqContext* ctx, const VqBlurParams* p, VqImage in, VqImage out, void* stream) { VQ_MARK("BlurY"); return blur_common(ctx, p, in, out, stream, true); }
+
+// All six faces of a one-mip cube, X then Y, in one launch: a CTA per face. The X pass reads the face from global memory and keeps
+// its result (RGB planes) in shared memory; after a barrier the Y pass reads those planes and stores the face. Both passes use the
+// tap sums of blur_x_kernel / blur_y_kernel with the same clamping, so each face equals vq_gaussian_blur_x -> vq_gaussian_blur_y.
+// A CTA reads only its own face, and all of it before it stores anything, so in == out (the same cube) is safe; the loads are
+// therefore plain (coherent) loads, not the read-only path.
+constexpr int BC_T = 1024;
+constexpr int BC_MAX_RES = 128;      // 3 planes x 128^2 x 4 B = 192 KB of shared memory (227 KB per CTA on H100)
+
+__global__ void __launch_bounds__(BC_T) blur_cube_kernel(const float4* in, float4* out, int res) {
+    extern __shared__ float sx[];    // [3][res * res]: the X pass of this face
+    const int n = res * res;
+    const float4* src = in + (size_t)blockIdx.x * n;
+    float4* dst = out + (size_t)blockIdx.x * n;
+    float* s0 = sx; float* s1 = sx + n; float* s2 = sx + 2 * n;
+    for (int i = threadIdx.x; i < n; i += BC_T) {
+        const int y = i / res, x = i - y * res;
+        const float4* row = src + (size_t)y * res;
+        const float3 a = gauss21_3([&](int k) { return xyz(row[min(max(x - 10 + k, 0), res - 1)]); });   // GaussianBlur.hlsl:144
+        s0[i] = a.x; s1[i] = a.y; s2[i] = a.z;
+    }
+    __syncthreads();                 // the whole face is read (in == out) and its X pass is in shared memory
+    for (int i = threadIdx.x; i < n; i += BC_T) {
+        const int y = i / res, x = i - y * res;
+        const float3 a = gauss21_3([&](int k) {
+            const int j = min(max(y - 10 + k, 0), res - 1) * res + x;                                       // GaussianBlur.hlsl:180
+            return f3(s0[j], s1[j], s2[j]);
+        });
+        st_stream(dst + i, make_float4(a.x, a.y, a.z, 1.0f));
+    }
+}
+
+extern "C" int vq_gaussian_blur_cube(VqContext* ctx, VqCubemap in, VqCubemap out, void* stream) {
+    VQ_REQUIRE(in.ptr && out.ptr, "null cubemap");
+    VQ_REQUIRE(in.mips == 1 && out.mips == 1, "blur cube: in and out must have exactly 1 mip");
+    VQ_REQUIRE(in.res >= 1 && in.res <= BC_MAX_RES, "blur cube: the face edge must be 1..128 (a face's X pass stays in shared memory)");
+    VQ_REQUIRE(out.res == in.res, "blur cube: in and out must have the same resolution");
+    VQ_REQUIRE(((uintptr_t)in.ptr % 16) == 0 && ((uintptr_t)out.ptr % 16) == 0, "blur cube: cubemaps must be 16-byte aligned");
+    const size_t bytes = (size_t)6 * in.res * in.res * sizeof(float4);
+    const uintptr_t a = (uintptr_t)in.ptr, b = (uintptr_t)out.ptr;
+    VQ_REQUIRE(a == b || a + bytes <= b || b + bytes <= a, "blur cube: in and out must be the same cube or not overlap");
+    const int rc = vq_enter(ctx); if (rc) return rc;
+    VQ_MARK("BlurDiffuseIrradianceCubemap");
+    const size_t smem = (size_t)3 * in.res * in.res * sizeof(float);
+    if (smem > 48 * 1024) VQ_CUDA_OK(cudaFuncSetAttribute(blur_cube_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    blur_cube_kernel<<<6, BC_T, smem, (cudaStream_t)stream>>>((const float4*)in.ptr, (float4*)out.ptr, in.res);
+    return vq_check_launch("gaussian_blur_cube");
+}
 
 // =============================================================================================
 // FidelityFX scalar helpers — FSR1.0/ffx_a.h:1842-1845 (integer bit tricks: reproduced exactly)

@@ -190,3 +190,54 @@ class InterleavedSpecularPlan:
             cube_t[a:b].view(self.world, k * n, *cube_t.shape[1:]).copy_(recv[:, off:off + k * n])
             off += k * n
         return cube_t
+
+
+def _signal_at(signal, epoch: int):
+    """a copy of the VqPeerSignal `signal` with `epoch` (None stays None: no rendezvous)"""
+    if signal is None:
+        return None
+    import ctypes as C
+    s = type(signal)()
+    C.memmove(C.addressof(s), C.addressof(signal), C.sizeof(s))
+    s.epoch = epoch & 0xFFFFFFFF
+    return s
+
+
+class EnvironmentStep:
+    """One rank's share of PreFilterEnvironmentMap across GPUs, with no collective library: every pass stores its band into every
+    rank's buffers over peer mappings, and the kernels' last CTAs run the rendezvous (DESIGN.md §6). In stream order:
+      1. diffuse(): K2 on this rank's rows of equal_tiles(6 * res, world) (every texel costs the same) into every rank's diffuse
+         cube, rendezvous with epoch e;
+      2. finish(): K5 on the local diffuse cube into the local blurred cube (one launch), then K3 on plan.row_ranges(rank) into
+         every rank's specular cube, rendezvous with epoch e + 1, then vq_environment_prepare of the local maps (when `env` is given).
+    run() is both; it returns the next free epoch, e + 2. The blurred cube must not be a peer destination of any call: the next
+    step's diffuse stores may land while this rank still reads its blurred cube."""
+
+    def __init__(self, ctx, hdri, diffuse_cubes, blurred, spec_cubes, rank: int, world: int, plan: "InterleavedSpecularPlan" = None,
+                 diffuse_params=None, num_samples: int = 512, env=None):
+        """diffuse_cubes / spec_cubes: Cubemap descriptors, the local one first, then the peers' mapped ones; blurred: the local
+        blurred diffuse cube; diffuse_params: the keyword arguments of Context.diffuse_irradiance (step, n_phi, n_theta, src_mip);
+        env: the local EnvironmentMaps to prepare after the step, or None"""
+        assert len(diffuse_cubes) == len(spec_cubes) == world and 0 <= rank < world
+        self.ctx, self.hdri, self.diffuse_cubes, self.blurred, self.spec_cubes = ctx, hdri, list(diffuse_cubes), blurred, list(spec_cubes)
+        self.rows = equal_tiles(6 * diffuse_cubes[0].res, world)[rank]
+        plan = plan if plan is not None else InterleavedSpecularPlan(spec_cubes[0].res, spec_cubes[0].mips, world)
+        self.spec_ranges = plan.row_ranges(rank)
+        self.diffuse_params = dict(diffuse_params or {})
+        self.num_samples, self.env = num_samples, env
+
+    def diffuse(self, epoch: int, signal=None, stream=None):
+        self.ctx.diffuse_irradiance_multi(self.hdri, self.diffuse_cubes, row_begin=self.rows[0], row_end=self.rows[1], stream=stream,
+                                          signal=_signal_at(signal, epoch), **self.diffuse_params)
+
+    def finish(self, epoch: int, signal=None, stream=None):
+        self.ctx.gaussian_blur_cube(self.diffuse_cubes[0], self.blurred, stream=stream)
+        self.ctx.specular_prefilter_ranges(self.hdri, self.spec_cubes, self.spec_ranges, self.num_samples,
+                                           signal=_signal_at(signal, epoch + 1), stream=stream)
+        if self.env is not None:
+            self.ctx.environment_prepare(self.env, stream=stream)
+
+    def run(self, epoch: int, signal=None, stream=None) -> int:
+        self.diffuse(epoch, signal, stream)
+        self.finish(epoch, signal, stream)
+        return epoch + 2
