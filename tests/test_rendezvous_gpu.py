@@ -22,10 +22,11 @@ comes back to its slot. So each retirement block also runs 320 signalled calls i
 Epoch 0xFFFFFFFF is left out, since its pre-set value e + 1 would wrap to 0, and only 0xFFFFFFFF itself satisfies an unsigned
 reading of it.
 
-Not tested, and why: the other direction of the wait, that a stale or wrapped flag must HOLD it, and the 20 s watchdog. Either
-needs a wait that may not be satisfied, whose failure on a shared GPU is a hang or a trap. So is a real multi-GPU step (NVLink
-peer stores, fence.sys ordering across devices): it needs two or more GPUs (tools/perf_multi_shading.py, tools/perf_post_multi.py
-under torchrun)."""
+The other direction of the wait, that a stale or wrapped flag must HOLD it, and ranks releasing each other while they run at the
+same time, are tested in tests/test_rendezvous_hold_gpu.py (flag arrays in mapped host memory, peers played by a host thread).
+Not tested: a real multi-GPU step (NVLink peer stores, fence.sys ordering across devices) needs two or more GPUs
+(tools/perf_multi_shading.py, tools/perf_post_multi.py under torchrun); the 20 s watchdog, on purpose, since testing it means a
+trap."""
 import ctypes as C
 import os
 import random
