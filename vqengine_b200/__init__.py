@@ -42,6 +42,9 @@ ABI_SYMBOLS = [
 ]
 # every symbol include/vqcuda_prefilter_multi.h declares (the environment prefilter across GPUs; vqcuda.h includes that header)
 PREFILTER_MULTI_SYMBOLS = ["vq_diffuse_irradiance_multi_signal", "vq_brdf_integration_lut_multi_signal", "vq_gaussian_blur_cube"]
+# every symbol include/vqcuda_group.h declares (the device group of a multi-GPU world in one process)
+GROUP_SYMBOLS = ["vq_group_create", "vq_group_destroy", "vq_group_rank_order", "vq_group_signal", "vq_group_arrive", "vq_band_rows",
+                 "vq_specular_rank_ranges"]
 
 
 class VqError(RuntimeError):
@@ -151,6 +154,13 @@ def _load() -> C.CDLL:
     lib.vq_depth_pyramid_texel_count.argtypes = [C.c_int, C.c_int, C.c_int]
     lib.vq_depth_pyramid_texel_count.restype = C.c_uint64
     lib.vq_depth_min_pyramid.argtypes = [vp, Image, vp, C.c_int, vp]
+    lib.vq_group_create.argtypes = [P(vp), C.c_int, P(vp), P(vp)]
+    lib.vq_group_destroy.argtypes = [vp]
+    lib.vq_group_rank_order.argtypes = [vp, C.c_int, P(C.c_int)]
+    lib.vq_group_signal.argtypes = [vp, C.c_int, u32, P(PeerSignal)]
+    lib.vq_group_arrive.argtypes = [vp, C.c_int, u32, vp]
+    lib.vq_band_rows.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int, P(C.c_int), P(C.c_int)]
+    lib.vq_specular_rank_ranges.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int, P(C.c_int), C.c_int, P(C.c_int)]
     return lib
 
 
@@ -258,6 +268,49 @@ def resize_axis_table(in_size: int, out_size: int):
     _check(lib.vq_resize_axis_table(in_size, out_size, start.ctypes.data_as(C.POINTER(C.c_int)), count.ctypes.data_as(C.POINTER(C.c_int)),
                                     w.ctypes.data_as(C.POINTER(f32)), mt.value, C.byref(mt)))
     return start, count, w
+
+
+# ---- the device group (include/vqcuda_group.h): band plans without a GPU, the group itself --------
+def band_rows(n_rows: int, n_ranks: int, rank: int, even: bool = False):
+    """vq_band_rows: rank `rank`'s [begin, end) rows of n_rows split over n_ranks (even: boundaries on even rows)"""
+    a, b = C.c_int(), C.c_int()
+    _check(lib.vq_band_rows(n_rows, n_ranks, rank, int(even), C.byref(a), C.byref(b)))
+    return a.value, b.value
+
+
+def specular_rank_ranges(res: int, mips: int, n_ranks: int, rank: int):
+    """vq_specular_rank_ranges: the [begin, end) rows of the flattened (mip, face, row) space rank `rank` prefilters"""
+    n = C.c_int()
+    r = (C.c_int * (2 * mips))()
+    _check(lib.vq_specular_rank_ranges(res, mips, n_ranks, rank, r, mips, C.byref(n)))
+    return [(r[2 * i], r[2 * i + 1]) for i in range(n.value)]
+
+
+class Group:
+    """vq_group_create over existing Contexts (rank r = contexts[r]); flag_arrays: None (the group allocates them) or one device
+    address per rank of n zeroed words that every rank's device can reach"""
+
+    def __init__(self, contexts, flag_arrays=None):
+        n = len(contexts)
+        ctxs = (C.c_void_p * max(n, 1))(*[c._h.value if isinstance(c, Context) else c for c in contexts])
+        flags = None if flag_arrays is None else (C.c_void_p * max(n, 1))(*flag_arrays)
+        self.n, self.h = n, C.c_void_p()
+        _check(lib.vq_group_create(ctxs, n, flags, C.byref(self.h)))
+
+    def rank_order(self, rank: int):
+        o = (C.c_int * 8)()
+        _check(lib.vq_group_rank_order(self.h, rank, o))
+        return list(o)
+
+    def signal(self, rank: int, epoch: int) -> PeerSignal:
+        s = PeerSignal()
+        _check(lib.vq_group_signal(self.h, rank, epoch & 0xFFFFFFFF, C.byref(s)))
+        return s
+
+    def close(self):
+        if self.h:
+            _check(lib.vq_group_destroy(self.h))
+            self.h = C.c_void_p()
 
 
 # ---- descriptors from torch tensors ------------------------------------------------------------

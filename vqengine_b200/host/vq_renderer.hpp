@@ -26,6 +26,7 @@
 #include <vector>
 
 #include "../../include/vqcuda.h"
+#include "../../include/vqcuda_group.h"
 
 typedef struct CUstream_st* cudaStream_t;
 
@@ -260,18 +261,99 @@ public:
     std::vector<unsigned char> SaveToHDRFileImage(const VqImage& Image);
 
     VqContext* Context() const { return mCtx; }
+    int Device() const { return mDevice; }
     const FTexture2D& SceneColor() const { return mSceneColor; }
     const FTexture2D& BRDFIntegrationLUT() const { return mBRDFLUT; }
 
 private:
+    friend class VQRendererGroup;   // binds each rank's targets and reuses the constant blocks and the post branch below
     void FillSceneConstants(const FSceneView& SceneView, const FPostProcessParameters& PPParams, const FEnvironmentMapRenderingResources& env,
                             const FGraphicsSettings& GFXSettings, bool bHDR, VqPerFrameData& PerFrame, VqPerViewLightingData& PerView) const;
+    VqEnvironmentMaps EnvironmentMaps(const FEnvironmentMapRenderingResources& env) const;   // the IBL SRVs PSMain binds
+    // RenderPostProcess's branch: the constant blocks of the passes that run (NULL: off) and the target they write
+    struct FPostPlan { VqTonemapperParams Tonemapper; const uint32_t *CAS, *EASU, *RCAS; VqImage Output; };
+    FPostPlan PlanPostProcess(const FPostProcessParameters& PPParams) const;
     VqContext* mCtx = nullptr;
+    int mDevice = 0;
     FTexture2D mBRDFLUT;                                        // EProceduralTextures::IBL_BRDF_INTEGRATION_LUT
     FTexture2D mSceneColor, mBlurTemp, mBlurOut;
     FTexture2D mPostOut;                                        // RenderPostProcess's output without FSR (render size)
     FTexture2D mRCASOut;                                        // ... with FSR (display size)
     VqImage mLastOutput{};
+};
+
+// ---- the renderer front end over a device group (vqcuda_group.h): one frame strong-scaled over several GPUs of one process ----
+// One VQRenderer per rank (its own context, BRDF LUT, scene colour and post targets, Rank(r)) and one non-blocking stream per rank
+// (Stream(r)). Each method runs the engine call of the same name across the group with the band forms of the passes underneath:
+// every rank computes its band and stores it into every rank's target, and the kernels' last CTAs meet (DESIGN.md §6), so every
+// rank ends each method holding the whole LUT, cube or frame. Inputs that live on a device come one per rank, in rank order
+// (G-buffers, surface inputs, material tables, shadow maps, environment resources, reflection radiance). The frame methods only
+// enqueue on the ranks' streams; LoadDefaultResources and PreFilterEnvironmentMap block, like the engine's.
+// Ranks may share a device (a simulated world: Initialize({0, 0})). Each rank's per-rank resources are made on its device:
+// call cudaSetDevice(Rank(r).Device()) before allocating them (FEnvironmentMapRenderingResources does that itself).
+class VQRendererGroup {
+public:
+    template <class T> using PerRank = std::vector<T>;
+    VQRendererGroup() = default;
+    ~VQRendererGroup() { Destroy(); }
+    VQRendererGroup(const VQRendererGroup&) = delete; VQRendererGroup& operator=(const VQRendererGroup&) = delete;
+
+    // one rank per entry of Devices (1..8); FlagArrays: nullptr -> the group allocates the flag words, else one caller-owned array
+    // of NumRanks words per rank that every rank's device can reach, all holding FirstEpoch - 1 (zero for the default)
+    bool Initialize(const std::vector<int>& Devices, uint32_t* const* FlagArrays = nullptr, uint32_t FirstEpoch = 1);
+    void Destroy();
+    int NumRanks() const { return (int)mRanks.size(); }
+    VQRenderer& Rank(int r) { return *mRanks[r]; }
+    cudaStream_t Stream(int r) const { return mStreams[r]; }
+    const VqGroup* Group() const { return mGroup; }
+    uint32_t Epoch() const { return mEpoch; }                  // the epoch the next signalled phase uses
+
+    bool LoadDefaultResources();                               // BLOCKS; each rank computes its band of the LUT into every LUT
+    // refused when a rank's scene band (even rows) or display band would be empty
+    bool OnWindowSizeChanged(int RenderW, int RenderH, int DisplayW, int DisplayH);
+    // BLOCKS. K2 band (epoch e) -> the cube blur locally -> K3 ranges (e + 1) -> vq_environment_prepare, on every rank; the frames
+    // below accept only the maps (cubes and LUT, as descriptors) the last call registered on each rank
+    bool PreFilterEnvironmentMap(const PerRank<FEnvironmentMapRenderingResources*>& envs, float DiffuseIntegrationStep = 0.010f);
+
+    // VQRenderer's four scene-colour calls on each rank's scene band. EnvironmentMapViewProj (nullptr: no sky) draws the skydome
+    // as the engine's RenderSceneColor does (SceneRendering.cpp:1821-1850): shading into the local frame, then the sky pass into
+    // every frame. Without a sky the shading call stores into every frame itself.
+    bool RenderSceneColor(const FSceneView& SceneView, const FPostProcessParameters& PPParams, const PerRank<VqGBuffer>& GBuffers,
+                          const PerRank<const FEnvironmentMapRenderingResources*>& envs, const FGraphicsSettings& GFXSettings,
+                          bool bHDR, const float* EnvironmentMapViewProj);
+    bool RenderSceneColorFromMaterials(const FSceneView& SceneView, const FPostProcessParameters& PPParams,
+                                       const PerRank<VqSurfaceInputs>& SurfaceInputs, const PerRank<const VqMaterialTable*>& MaterialTables,
+                                       const PerRank<const FEnvironmentMapRenderingResources*>& envs, const FGraphicsSettings& GFXSettings,
+                                       bool bHDR, const float* EnvironmentMapViewProj, bool bAlphaMask = false);
+    bool RenderSceneColor(const FSceneView& SceneView, const FPostProcessParameters& PPParams, const PerRank<VqGBuffer>& GBuffers,
+                          const PerRank<const FEnvironmentMapRenderingResources*>& envs, const FGraphicsSettings& GFXSettings,
+                          bool bHDR, const PerRank<VqShadowMaps>& ShadowMaps, const float* EnvironmentMapViewProj);
+    bool RenderSceneColorFromMaterials(const FSceneView& SceneView, const FPostProcessParameters& PPParams,
+                                       const PerRank<VqSurfaceInputs>& SurfaceInputs, const PerRank<const VqMaterialTable*>& MaterialTables,
+                                       const PerRank<const FEnvironmentMapRenderingResources*>& envs, const FGraphicsSettings& GFXSettings,
+                                       bool bHDR, const PerRank<VqShadowMaps>& ShadowMaps, const float* EnvironmentMapViewProj,
+                                       bool bAlphaMask = false);
+    bool ApplyReflections(const PerRank<VqImage>& ReflectionRadiance, const PerRank<VqImage>* BoundingVolumes = nullptr);
+    // each rank's display frame (NumRanks() images, rank r at [r]); nullptr when refused. The Gaussian blur has no band form and
+    // is refused.
+    const VqImage* RenderPostProcess(const FPostProcessParameters& PPParams, bool bHDR);
+
+private:
+    struct FSceneCall;
+    bool RenderScene(const FSceneCall& call);
+    // one signalled phase: issue(r) on every rank in order; if a rank refuses, the ranks from it on arrive at `epoch` in their
+    // peers' flag arrays (vq_group_arrive), so that the ranks already enqueued finish instead of waiting for them
+    template <class F> bool Phase(uint32_t epoch, F issue);
+    std::vector<VqImage> Targets(int r, const FTexture2D VQRenderer::* member) const;   // rank r's destinations in its rank order
+    bool Prepared(const PerRank<const FEnvironmentMapRenderingResources*>& envs) const;
+
+    std::vector<std::unique_ptr<VQRenderer>> mRanks;
+    std::vector<cudaStream_t> mStreams;
+    std::vector<VqEnvironmentMaps> mPrepared;                  // the maps vq_environment_prepare registered, per rank (ptr 0: none)
+    std::vector<VqImage> mDisplay;
+    VqGroup* mGroup = nullptr;
+    uint32_t mEpoch = 1;
+    std::vector<char> mShadowRecordsSized;                     // per rank: a PCF test has sized the records at this size (rule 3, DESIGN §6)
 };
 
 }  // namespace vq
