@@ -140,7 +140,9 @@ VQ_API uint64_t vq_launch_count(void);
  * until words j != my_index of its OWN array have reached `epoch` — i.e. until every peer has finished storing into this
  * rank's buffers. flags[0] = this rank's array, flags[1..n_ranks-1] = the peers' arrays mapped into this process
  * (n_ranks 32-bit words each, zero-initialised, e.g. in torch symmetric memory); epoch must increase from call to call.
- * Replaces a host-issued barrier per step: the step is ONE kernel. */
+ * Replaces a host-issued barrier per step: the step is ONE kernel. A peer that never arrives fails the kernel after 20 s (a trap)
+ * unless the calling context registered a deadline (vqcuda_rendezvous.h): the wait then ends at the deadline or on a cancel and
+ * is recorded in the context's status instead. */
 typedef struct VqPeerSignal {
     uint32_t* flags[8];
     int32_t   n_ranks;

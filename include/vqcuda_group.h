@@ -13,6 +13,7 @@
 #define VQCUDA_GROUP_H
 
 #include "vqcuda.h"
+#include "vqcuda_rendezvous.h"
 
 #ifdef __cplusplus
 extern "C" {
@@ -40,6 +41,19 @@ VQ_API int vq_group_signal(const VqGroup* g, int rank, uint32_t epoch, VqPeerSig
  * phase was refused after its peers' calls were enqueued: the peers finish instead of waiting for it. The result of that phase is
  * invalid. Refused: a null group, rank out of range. */
 VQ_API int vq_group_arrive(const VqGroup* g, int rank, uint32_t epoch, void* stream);
+
+/* The rendezvous policy of vqcuda_rendezvous.h on every rank's context: a deadline of `ns` (1..VQ_RENDEZVOUS_MAX_DEADLINE_NS) for
+ * the signalled calls enqueued after this returns. Refused: a null group, ns outside the range. */
+VQ_API int vq_group_set_rendezvous_deadline(const VqGroup* g, uint64_t ns);
+/* vq_ctx_cancel_rendezvous on every rank's context (a host store each, no CUDA call). Refused: a null group, a rank whose context
+ * has no registered deadline. */
+VQ_API int vq_group_cancel(const VqGroup* g);
+/* Rank `rank`'s rendezvous at `epoch` without a pass, after all work enqueued earlier on `stream`: one one-thread launch on the
+ * rank's device that stores `epoch` into word `rank` of every peer's flag array and waits, under the rank's policy, until every
+ * peer's word in its own array has reached `epoch`. Every rank's barrier at a fresh epoch is how a group meets again after a wait
+ * gave up: once every rank's barrier has met its peers, every store of the earlier steps, a late peer's included, has landed.
+ * A group of one rank launches nothing. Refused: a null group, rank out of range. */
+VQ_API int vq_group_barrier(const VqGroup* g, int rank, uint32_t epoch, void* stream);
 
 /* HOST. The rows [*row_begin, *row_end) of rank `rank` when n_rows rows are split over n_ranks ranks:
  *   even = 0: contiguous blocks whose sizes differ by at most one, rank r from floor(n_rows r / n) (the shading of a G-buffer,

@@ -1,6 +1,6 @@
 """GPU-box helper: the C++ front end's device group (vq::VQRendererGroup) against the single vq::VQRenderer.
 
-  python tools/perf_group.py [--frames 200] [--w 1920] [--h 1080]
+  python tools/perf_group.py [--frames 200] [--w 1920] [--h 1080] [--deadline-ns NS [--ranks 1,3]]
 
 Builds a small timing program against libvqhost.so in a temporary directory and runs it. Workload: vq_headless_test's scene at the
 given render size (a synthetic G-buffer, a 512x256 HDRI, a 64 diffuse / 128 specular cube), RenderSceneColor with the sky,
@@ -12,6 +12,8 @@ it is the host clock around the call, which ends in a synchronise of every rank'
   * a 1-rank group against VQRenderer (the group's own cost);
   * N = 2, 4, 8 ranks on device 0 (a simulated world: a cost figure, not a scaling figure);
   * with two or more GPUs, 1/2/4/8-rank strong scaling over real devices.
+With --deadline-ns, each group of --ranks ranks on device 0 runs alternately without and with that rendezvous deadline registered
+(vqcuda_rendezvous.h), --repeats times each, so that the cost of the policy in the wait loop shows against the run-to-run spread.
 The card's name and power limit are read in the same run."""
 import argparse, json, os, statistics, subprocess, sys, tempfile
 
@@ -31,11 +33,13 @@ using Clock = std::chrono::steady_clock;
 static double ms(Clock::time_point a) { return std::chrono::duration<double, std::milli>(Clock::now() - a).count(); }
 int main(int argc, char** argv) {
     const int frames = std::atoi(argv[1]), W = std::atoi(argv[2]), H = std::atoi(argv[3]);
-    std::vector<int> dev; for (int i = 4; i < argc; ++i) dev.push_back(std::atoi(argv[i]));
+    const unsigned long long deadline = std::strtoull(argv[4], nullptr, 10);     // 0: none registered
+    std::vector<int> dev; for (int i = 5; i < argc; ++i) dev.push_back(std::atoi(argv[i]));
     const bool single = dev.empty();
     const int n = single ? 1 : (int)dev.size();
     vq::VQRenderer R; vq::VQRendererGroup G;
-    if (single ? !R.Initialize(0) || !R.LoadDefaultResources() : !G.Initialize(dev) || !G.LoadDefaultResources()) return 2;
+    if (single ? !R.Initialize(0) || !R.LoadDefaultResources()
+               : !G.Initialize(dev) || (deadline && !G.SetRendezvousDeadline(deadline)) || !G.LoadDefaultResources()) return 2;
     const int EW = 512, EH = 256;
     std::vector<float> hdri((size_t)EW * EH * 4);
     for (size_t i = 0; i < hdri.size(); ++i) hdri[i] = 0.2f + 1.5f * std::fabs(std::sin(0.001f * (float)i));
@@ -111,7 +115,9 @@ int main(int argc, char** argv) {
         cudaEventElapsedTime(&t, start[r], end[r]);
         worst = t > worst ? t : worst;
     }
-    std::printf("{\"ranks\": %d, \"single_renderer\": %s, \"frame_ms\": %.4f, \"prefilter_ms\": %.4f}\n", n, single ? "true" : "false", worst / frames, pre);
+    if (!single && !G.RendezvousOK()) return 6;
+    std::printf("{\"ranks\": %d, \"single_renderer\": %s, \"deadline_ns\": %llu, \"frame_ms\": %.4f, \"prefilter_ms\": %.4f}\n", n,
+                single ? "true" : "false", deadline, worst / frames, pre);
     cudaStreamDestroy(s);
     for (auto& e : envs) e.DestroyRenderingResources();
     return 0;
@@ -125,6 +131,8 @@ def main():
     ap.add_argument("--w", type=int, default=1920)
     ap.add_argument("--h", type=int, default=1080)
     ap.add_argument("--repeats", type=int, default=3)
+    ap.add_argument("--deadline-ns", type=int, default=0, help="compare groups without and with this rendezvous deadline")
+    ap.add_argument("--ranks", default="1,3", help="with --deadline-ns: the group sizes on device 0")
     a = ap.parse_args()
     import torch
     assert torch.cuda.is_available(), "perf_group.py needs a CUDA device"
@@ -138,19 +146,32 @@ def main():
                                f"-Wl,-rpath,{lib}", f"-Wl,-rpath,{os.path.join(cuda, 'lib64')}", "-o", exe])
         env = dict(os.environ, CUDA_DEVICE_MAX_CONNECTIONS="32")
 
-        def run(devices):
-            reps = []
-            for _ in range(a.repeats):
-                out = subprocess.run([exe, str(a.frames), str(a.w), str(a.h), *map(str, devices)], capture_output=True, text=True,
-                                     env=env, timeout=1200)
-                assert out.returncode == 0, out.stdout + out.stderr
-                reps.append(json.loads(out.stdout.strip().splitlines()[-1]))
+        def once(devices, deadline=0):
+            out = subprocess.run([exe, str(a.frames), str(a.w), str(a.h), str(deadline), *map(str, devices)], capture_output=True, text=True,
+                                 env=env, timeout=1200)
+            assert out.returncode == 0, out.stdout + out.stderr
+            return json.loads(out.stdout.strip().splitlines()[-1])
+
+        def summary(reps):
             spread = lambda k: [round(v, 4) for v in (min(x[k] for x in reps), statistics.median(x[k] for x in reps), max(x[k] for x in reps))]
-            return {"ranks": reps[0]["ranks"], "single_renderer": reps[0]["single_renderer"],
+            return {"ranks": reps[0]["ranks"], "single_renderer": reps[0]["single_renderer"], "deadline_ns": reps[0]["deadline_ns"],
                     "frame_ms_min_median_max": spread("frame_ms"), "prefilter_ms_min_median_max": spread("prefilter_ms")}
+
+        def run(devices):
+            return summary([once(devices) for _ in range(a.repeats)])
 
         card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True,
                               text=True).stdout.strip().splitlines()
+        if a.deadline_ns:
+            res = {"card": card, "size": [a.w, a.h], "frames": a.frames, "deadline": []}
+            for k in (int(x) for x in a.ranks.split(",")):
+                without, with_ = [], []
+                for _ in range(a.repeats):                  # alternated, so that both see the same drift of a shared host
+                    without.append(once([0] * k))
+                    with_.append(once([0] * k, a.deadline_ns))
+                res["deadline"].append({"without": summary(without), "with": summary(with_)})
+            print(json.dumps(res))
+            return
         res = {"card": card, "size": [a.w, a.h], "frames": a.frames, "single": run([]), "one_device": [run([0] * k) for k in (1, 2, 4, 8)]}
         ngpu = torch.cuda.device_count()
         if ngpu >= 2:

@@ -44,7 +44,19 @@ ABI_SYMBOLS = [
 PREFILTER_MULTI_SYMBOLS = ["vq_diffuse_irradiance_multi_signal", "vq_brdf_integration_lut_multi_signal", "vq_gaussian_blur_cube"]
 # every symbol include/vqcuda_group.h declares (the device group of a multi-GPU world in one process)
 GROUP_SYMBOLS = ["vq_group_create", "vq_group_destroy", "vq_group_rank_order", "vq_group_signal", "vq_group_arrive", "vq_band_rows",
-                 "vq_specular_rank_ranges"]
+                 "vq_specular_rank_ranges", "vq_group_set_rendezvous_deadline", "vq_group_cancel", "vq_group_barrier"]
+# every symbol include/vqcuda_rendezvous.h declares (a context's deadline, cancel and status record for the in-kernel rendezvous)
+RENDEZVOUS_SYMBOLS = ["vq_ctx_set_rendezvous_deadline", "vq_ctx_cancel_rendezvous", "vq_ctx_rendezvous_status",
+                      "vq_ctx_rendezvous_clear"]
+RENDEZVOUS_MAX_DEADLINE_NS = 20_000_000_000
+
+
+class RendezvousStatus(C.Structure):
+    """VqRendezvousStatus (vqcuda_rendezvous.h): the waits of a context that gave up since the last clear"""
+    _fields_ = [("failures", u32), ("first_epoch", u32), ("last_epoch", u32), ("missing_mask", u32), ("cancelled", u32)]
+
+    def missing_ranks(self):
+        return [j for j in range(8) if self.missing_mask >> j & 1]
 
 
 class VqError(RuntimeError):
@@ -159,6 +171,13 @@ def _load() -> C.CDLL:
     lib.vq_group_rank_order.argtypes = [vp, C.c_int, P(C.c_int)]
     lib.vq_group_signal.argtypes = [vp, C.c_int, u32, P(PeerSignal)]
     lib.vq_group_arrive.argtypes = [vp, C.c_int, u32, vp]
+    lib.vq_group_set_rendezvous_deadline.argtypes = [vp, C.c_uint64]
+    lib.vq_group_cancel.argtypes = [vp]
+    lib.vq_group_barrier.argtypes = [vp, C.c_int, u32, vp]
+    lib.vq_ctx_set_rendezvous_deadline.argtypes = [vp, C.c_uint64]
+    lib.vq_ctx_cancel_rendezvous.argtypes = [vp]
+    lib.vq_ctx_rendezvous_status.argtypes = [vp, vp, P(RendezvousStatus)]
+    lib.vq_ctx_rendezvous_clear.argtypes = [vp, vp]
     lib.vq_band_rows.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int, P(C.c_int), P(C.c_int)]
     lib.vq_specular_rank_ranges.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int, P(C.c_int), C.c_int, P(C.c_int)]
     return lib
@@ -307,6 +326,18 @@ class Group:
         _check(lib.vq_group_signal(self.h, rank, epoch & 0xFFFFFFFF, C.byref(s)))
         return s
 
+    def set_rendezvous_deadline(self, ns: int):
+        """Context.set_rendezvous_deadline on every rank's context"""
+        _check(lib.vq_group_set_rendezvous_deadline(self.h, ns))
+
+    def cancel(self):
+        """Context.cancel_rendezvous on every rank's context"""
+        _check(lib.vq_group_cancel(self.h))
+
+    def barrier(self, rank: int, epoch: int, stream=None):
+        """vq_group_barrier: rank `rank` meets its peers at `epoch` with no pass, after the work enqueued on `stream`"""
+        _check(lib.vq_group_barrier(self.h, rank, epoch & 0xFFFFFFFF, _stream_ptr(stream)))
+
     def close(self):
         if self.h:
             _check(lib.vq_group_destroy(self.h))
@@ -395,6 +426,23 @@ class Context:
 
     def resize(self, w: int, h: int):
         _check(lib.vq_ctx_resize(self._h, w, h))
+
+    # the rendezvous policy (vqcuda_rendezvous.h): a signalled call whose peer does not arrive ends at the deadline, or when the
+    # host cancels, and records it here instead of trapping after 20 s
+    def set_rendezvous_deadline(self, ns: int):
+        _check(lib.vq_ctx_set_rendezvous_deadline(self._h, ns))
+
+    def cancel_rendezvous(self):
+        _check(lib.vq_ctx_cancel_rendezvous(self._h))
+
+    def rendezvous_status(self, stream=None) -> RendezvousStatus:
+        """blocking: the record after the work enqueued on `stream` (default: torch's current stream)"""
+        st = RendezvousStatus()
+        _check(lib.vq_ctx_rendezvous_status(self._h, _stream_ptr(stream), C.byref(st)))
+        return st
+
+    def clear_rendezvous_status(self, stream=None):
+        _check(lib.vq_ctx_rendezvous_clear(self._h, _stream_ptr(stream)))
 
     # K1
     def forward_lighting(self, per_frame, per_view, gbuffer: GBuffer, env: EnvironmentMaps, out, row_begin=0,

@@ -47,13 +47,21 @@ int vq_scratch_reserve(VqScratch& s, size_t need, const char* what) {
     return VQ_OK;
 }
 
-int vq_fill_peer_sync(const VqPeerSignal* sig, PeerSync* out) {
+int vq_fill_peer_sync(const VqContext* ctx, const VqPeerSignal* sig, PeerSync* out) {
     memset(out, 0, sizeof(*out));
     if (!sig || sig->n_ranks <= 1) return VQ_OK;
     VQ_REQUIRE(sig->n_ranks <= 8 && sig->my_index >= 0 && sig->my_index < sig->n_ranks, "bad peer signal descriptor");
     for (int k = 0; k < sig->n_ranks; ++k) { VQ_REQUIRE(sig->flags[k], "null flag array in the peer signal"); out->flags[k] = sig->flags[k]; }
     out->n = sig->n_ranks; out->myIndex = sig->my_index; out->epoch = sig->epoch;
+    const uint64_t deadline = ctx ? ctx->rv_deadline_ns.load(std::memory_order_acquire) : 0;
+    if (deadline) { out->deadlineNs = deadline; out->cancel = ctx->rv_cancel_dev; out->status = ctx->rv_status; }
     return VQ_OK;
+}
+
+// vq_ctx_rendezvous_clear: the record and the cancel word zeroed in stream order (loaded when the first deadline is registered)
+__global__ void rendezvous_clear_kernel(VqRendezvousStatus* status, uint32_t* cancel) {
+    *status = VqRendezvousStatus{};
+    asm volatile("st.relaxed.sys.global.u32 [%0], %1;" :: "l"(cancel), "r"(0u) : "memory");
 }
 
 extern "C" {
@@ -101,9 +109,75 @@ int vq_ctx_destroy(VqContext* ctx) {
         for (auto& e : ctx->events) cudaEventDestroy(e);
     }
     if (ctx->spd_counter) cudaFree(ctx->spd_counter);
+    if (ctx->rv_status) cudaFree(ctx->rv_status);
+    if (ctx->rv_cancel_host) cudaFreeHost((void*)ctx->rv_cancel_host);
     delete ctx->spd_next; delete ctx->mu;
     delete ctx;                 // frees the scratch (~VqScratch)
     return VQ_OK;
+}
+
+// ---- the rendezvous policy (vqcuda_rendezvous.h) ------------------------------------------------
+int vq_ctx_set_rendezvous_deadline(VqContext* ctx, uint64_t ns) {
+    VQ_REQUIRE(ctx, "null context");
+    VQ_REQUIRE(ns >= 1 && ns <= VQ_RENDEZVOUS_MAX_DEADLINE_NS, "the deadline must be 1 ns..20 s");
+    int rc = vq_enter(ctx); if (rc) return rc;
+    VqScratchLock lock(ctx);
+    if (!ctx->rv_status) {
+        cudaFuncAttributes attr;       // a first launch loads its module, which would wait for the signalled kernels running then
+        VQ_CUDA_OK(cudaFuncGetAttributes(&attr, rendezvous_clear_kernel));
+        void* host = nullptr;
+        void* dev = nullptr;
+        VqRendezvousStatus* status = nullptr;
+        cudaError_t e = cudaHostAlloc(&host, sizeof(uint32_t), cudaHostAllocMapped | cudaHostAllocPortable);
+        if (e == cudaSuccess) { *(volatile uint32_t*)host = 0u; e = cudaHostGetDevicePointer(&dev, host, 0); }
+        if (e == cudaSuccess) e = cudaMalloc(&status, sizeof(VqRendezvousStatus));
+        // the zeroes land before any call of any stream reads them, without waiting for the rest of the device: a stream of its own
+        cudaStream_t zs = nullptr;
+        if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&zs, cudaStreamNonBlocking);
+        if (e == cudaSuccess) e = cudaMemsetAsync(status, 0, sizeof(VqRendezvousStatus), zs);
+        if (e == cudaSuccess) e = cudaStreamSynchronize(zs);
+        if (zs) cudaStreamDestroy(zs);
+        if (e != cudaSuccess) {
+            cudaGetLastError();
+            if (status) cudaFree(status);
+            if (host) cudaFreeHost(host);
+            vq_set_error("rendezvous status and cancel word: %s", cudaGetErrorString(e));
+            return e == cudaErrorMemoryAllocation ? VQ_ERR_OUT_OF_MEMORY : VQ_ERR_CUDA;
+        }
+        ctx->rv_cancel_host = (volatile uint32_t*)host;
+        ctx->rv_cancel_dev = (const uint32_t*)dev;
+        ctx->rv_status = status;
+    }
+    ctx->rv_deadline_ns.store(ns, std::memory_order_release);
+    return VQ_OK;
+}
+
+int vq_ctx_cancel_rendezvous(VqContext* ctx) {
+    VQ_REQUIRE(ctx, "null context");
+    VQ_REQUIRE(ctx->rv_deadline_ns.load(std::memory_order_acquire) != 0, "no rendezvous deadline is registered on this context");
+    __atomic_store_n(ctx->rv_cancel_host, 1u, __ATOMIC_RELEASE);
+    return VQ_OK;
+}
+
+int vq_ctx_rendezvous_status(VqContext* ctx, void* stream, VqRendezvousStatus* out) {
+    VQ_REQUIRE(ctx, "null context");
+    VQ_REQUIRE(out, "out is null");
+    memset(out, 0, sizeof(*out));
+    if (ctx->rv_deadline_ns.load(std::memory_order_acquire) == 0) return VQ_OK;
+    int rc = vq_enter(ctx); if (rc) return rc;
+    VqRendezvousStatus s;          // pageable: the copy has completed when the call returns
+    VQ_CUDA_OK(cudaMemcpyAsync(&s, ctx->rv_status, sizeof(s), cudaMemcpyDeviceToHost, (cudaStream_t)stream));
+    VQ_CUDA_OK(cudaStreamSynchronize((cudaStream_t)stream));
+    *out = s;
+    return VQ_OK;
+}
+
+int vq_ctx_rendezvous_clear(VqContext* ctx, void* stream) {
+    VQ_REQUIRE(ctx, "null context");
+    if (ctx->rv_deadline_ns.load(std::memory_order_acquire) == 0) return VQ_OK;
+    int rc = vq_enter(ctx); if (rc) return rc;
+    rendezvous_clear_kernel<<<1, 1, 0, (cudaStream_t)stream>>>(ctx->rv_status, (uint32_t*)ctx->rv_cancel_dev);
+    return vq_check_launch("rendezvous_clear");
 }
 
 // ---- packed layouts ---------------------------------------------------------------------------

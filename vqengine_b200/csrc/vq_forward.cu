@@ -1082,8 +1082,8 @@ static int frame_params(VqContext* ctx, const VqPerFrameData* pf, const VqPerVie
 // The destinations, row range and rendezvous of a multi-destination call over a W x H source (G-buffer or attribute planes):
 // 1..8 frames as wide as the source that hold dst_row_offset + H rows, rows inside the source, a signal only with peer
 // destinations and rows to shade (its last CTA runs the rendezvous). Host-side only; fills `sync` from `sig`.
-int vq_multi_dest_check(const VqImage* outs, int n_outs, int W, int H, int dst_row_offset, int row_begin, int row_end,
-                        const VqPeerSignal* sig, PeerSync& sync) {
+int vq_multi_dest_check(const VqContext* ctx, const VqImage* outs, int n_outs, int W, int H, int dst_row_offset, int row_begin,
+                        int row_end, const VqPeerSignal* sig, PeerSync& sync) {
     VQ_REQUIRE(n_outs >= 1 && n_outs <= 8, "1..8 destinations");
     VQ_REQUIRE(dst_row_offset >= 0, "negative destination row offset");
     for (int k = 0; k < n_outs; ++k)
@@ -1091,7 +1091,7 @@ int vq_multi_dest_check(const VqImage* outs, int n_outs, int W, int H, int dst_r
                    "every destination must be as wide as the G-buffer and hold dst_row_offset + height rows");
     VQ_REQUIRE(row_begin >= 0 && row_end <= H && row_begin <= row_end, "row range out of bounds");
     VQ_REQUIRE(row_begin < row_end || !(sig && sig->n_ranks > 1), "a rendezvous needs a non-empty row range (the kernel runs it)");
-    const int rc = vq_fill_peer_sync(sig, &sync); if (rc) return rc;
+    const int rc = vq_fill_peer_sync(ctx, sig, &sync); if (rc) return rc;
     VQ_REQUIRE(sync.n == 0 || n_outs > 1, "a rendezvous only makes sense with peer destinations");
     return VQ_OK;
 }
@@ -1106,7 +1106,7 @@ int vq_forward_launch_multi(VqContext* ctx, const VqPerFrameData* pf, const VqPe
     VQ_REQUIRE(gb->normal_roughness.width == W && gb->albedo_metalness.width == W &&
                gb->normal_roughness.height == H && gb->albedo_metalness.height == H, "G-buffer planes must have the same size");
     PeerSync sync;
-    int rc = vq_multi_dest_check(outs, n_outs, W, H, dst_row_offset, row_begin, row_end, sig, sync); if (rc) return rc;
+    int rc = vq_multi_dest_check(ctx, outs, n_outs, W, H, dst_row_offset, row_begin, row_end, sig, sync); if (rc) return rc;
     const VqSceneLighting& L = pf->Lights;
     VQ_REQUIRE(light_counts_ok(L), "light counts exceed the cbuffer arrays");
     if (row_begin == row_end) return VQ_OK;
@@ -1218,7 +1218,7 @@ static int psmain_launch(VqContext* ctx, const VqPerFrameData* pf, const VqPerVi
     memset(&Q, 0, sizeof(Q));
     int rc;
     if (multi) {
-        rc = vq_multi_dest_check(outs, n_outs, W, H, dst_row_offset, row_begin, row_end, sig, Q.F.sync); if (rc) return rc;
+        rc = vq_multi_dest_check(ctx, outs, n_outs, W, H, dst_row_offset, row_begin, row_end, sig, Q.F.sync); if (rc) return rc;
         // the surface producer's quads sit on even rows of the attribute planes: an even offset keeps them on even rows of the frame
         VQ_REQUIRE((dst_row_offset & 1) == 0, "dst_row_offset must be even (quads are aligned to even rows)");
     } else {

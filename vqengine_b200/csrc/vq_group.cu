@@ -1,6 +1,7 @@
 // vq_group.cu — the device group of vqcuda_group.h: peer access, flag arrays, rank orders and signals of a multi-GPU world in
 // one process, and the band plans (the row splits that vqengine_b200/distributed.py's equal_tiles, even_tiles and
-// InterleavedSpecularPlan compute for the torch path). One kernel: the arrival of a rank whose signalled call was refused.
+// InterleavedSpecularPlan compute for the torch path). Two kernels: the arrival of a rank whose signalled call was refused, and the
+// barrier of a rank with no pass.
 #include "vq_common.cuh"
 #include "../../include/vqcuda_group.h"
 
@@ -9,6 +10,7 @@
 struct VqGroup {
     int n = 0;
     int device[8] = {};
+    VqContext* ctx[8] = {};           // rank r's context: its rendezvous policy (vqcuda_rendezvous.h)
     uint32_t* flags[8] = {};
     bool owned = false;              // the flag arrays are the group's (cudaMalloc on each rank's device)
 };
@@ -18,6 +20,19 @@ __global__ void group_arrive_kernel(PeerSync y) {
     __threadfence_system();
     for (int k = 1; k < y.n; ++k)
         asm volatile("st.release.sys.global.u32 [%0], %1;" :: "l"(y.flags[k] + y.myIndex), "r"(y.epoch) : "memory");
+}
+
+// one thread: a signalled call's rendezvous without its pass (the epoch into the peers' arrays, then the wait under the rank's policy)
+__global__ void group_barrier_kernel(const PeerSync y) {
+    __threadfence_system();
+    vq::peer_rendezvous(y);
+}
+
+// rank r's PeerSync at `epoch` (vq_group_signal's flag arrays and the rank's policy)
+static int group_peer_sync(const VqGroup* g, int rank, uint32_t epoch, PeerSync* y) {
+    VqPeerSignal sig;
+    vq_group_signal(g, rank, epoch, &sig);
+    return vq_fill_peer_sync(g->ctx[rank], &sig, y);
 }
 
 static void vq_group_free_flags(VqGroup* g) {
@@ -56,17 +71,18 @@ int vq_group_create(VqContext* const* ctxs, int n_ranks, uint32_t* const* flag_a
             if (e == cudaErrorPeerAccessAlreadyEnabled) { cudaGetLastError(); continue; }
             VQ_CUDA_OK(e);
         }
-    // load the arrival kernel on every rank's device now: a first launch loads its module, and a module load waits for the kernels
-    // already running, which include the signalled calls the arrival would release
+    // load the arrival and barrier kernels on every rank's device now: a first launch loads its module, and a module load waits for
+    // the kernels already running, which include the signalled calls the arrival would release
     for (int r = 0; r < n_ranks; ++r) {
         cudaFuncAttributes attr;
         VQ_CUDA_OK(cudaSetDevice(dev[r]));
         VQ_CUDA_OK(cudaFuncGetAttributes(&attr, group_arrive_kernel));
+        VQ_CUDA_OK(cudaFuncGetAttributes(&attr, group_barrier_kernel));
     }
     VqGroup* g = new (std::nothrow) VqGroup();
     if (!g) { vq_set_error("out of host memory"); return VQ_ERR_OUT_OF_MEMORY; }
     g->n = n_ranks;
-    for (int r = 0; r < n_ranks; ++r) g->device[r] = dev[r];
+    for (int r = 0; r < n_ranks; ++r) { g->device[r] = dev[r]; g->ctx[r] = ctxs[r]; }
     if (flag_arrays) {
         for (int r = 0; r < n_ranks; ++r) g->flags[r] = flag_arrays[r];
     } else {
@@ -128,6 +144,33 @@ int vq_group_arrive(const VqGroup* g, int rank, uint32_t epoch, void* stream) {
     VQ_CUDA_OK(cudaSetDevice(g->device[rank]));
     group_arrive_kernel<<<1, 1, 0, (cudaStream_t)stream>>>(y);
     return vq_check_launch("group_arrive");
+}
+
+int vq_group_set_rendezvous_deadline(const VqGroup* g, uint64_t ns) {
+    VQ_REQUIRE(g, "null group");
+    VQ_REQUIRE(ns >= 1 && ns <= VQ_RENDEZVOUS_MAX_DEADLINE_NS, "the deadline must be 1 ns..20 s");
+    for (int r = 0; r < g->n; ++r) { const int rc = vq_ctx_set_rendezvous_deadline(g->ctx[r], ns); if (rc) return rc; }
+    return VQ_OK;
+}
+
+int vq_group_cancel(const VqGroup* g) {
+    VQ_REQUIRE(g, "null group");
+    // every rank checked before any is cancelled: a refusal cancels nothing
+    for (int r = 0; r < g->n; ++r)
+        VQ_REQUIRE(g->ctx[r]->rv_deadline_ns.load(std::memory_order_acquire) != 0, "a rank's context has no rendezvous deadline registered");
+    for (int r = 0; r < g->n; ++r) { const int rc = vq_ctx_cancel_rendezvous(g->ctx[r]); if (rc) return rc; }
+    return VQ_OK;
+}
+
+int vq_group_barrier(const VqGroup* g, int rank, uint32_t epoch, void* stream) {
+    VQ_REQUIRE(g, "null group");
+    VQ_REQUIRE(rank >= 0 && rank < g->n, "rank out of range");
+    if (g->n == 1) return VQ_OK;
+    PeerSync y;
+    int rc = group_peer_sync(g, rank, epoch, &y); if (rc) return rc;
+    VQ_CUDA_OK(cudaSetDevice(g->device[rank]));
+    group_barrier_kernel<<<1, 1, 0, (cudaStream_t)stream>>>(y);
+    return vq_check_launch("group_barrier");
 }
 
 int vq_band_rows(int n_rows, int n_ranks, int rank, int even, int* row_begin, int* row_end) {

@@ -441,7 +441,7 @@ extern "C" int vq_diffuse_irradiance_multi_signal(VqContext* ctx, const VqDiffus
         VQ_REQUIRE(outs[k].ptr != outs[0].ptr, "a peer destination must not be the local cubemap outs[0]");
     }
     VQ_REQUIRE(row_begin < row_end || !(signal && signal->n_ranks > 1), "a rendezvous needs a non-empty row range (the kernel runs it)");
-    rc = vq_fill_peer_sync(signal, &M.sync); if (rc) return rc;
+    rc = vq_fill_peer_sync(ctx, signal, &M.sync); if (rc) return rc;
     VQ_REQUIRE(M.sync.n == 0 || n_outs > 1, "a rendezvous only makes sense with peer destinations");
     rc = vq_enter(ctx); if (rc) return rc;
     VQ_MARK("DiffuseIrradianceCubemap");
@@ -493,7 +493,7 @@ static int specular_launch(VqContext* ctx, VqPyramid hd, const VqCubemap* outs, 
             mipRow0 += rows;
         }
     }
-    { const int rcs = vq_fill_peer_sync(sig, &W.sync); if (rcs) return rcs; }
+    { const int rcs = vq_fill_peer_sync(ctx, sig, &W.sync); if (rcs) return rcs; }
     if (units == 0 && W.sync.n == 0) return VQ_OK;
     // segments must be visited in increasing unit order with mips that only change forward per CTA: sort is implied by the
     // increasing ranges; roughness 0 segments may sit between others, which only costs a table rebuild
@@ -578,7 +578,7 @@ extern "C" int vq_brdf_integration_lut_multi_signal(VqContext* ctx, const VqImag
     VQ_REQUIRE(row_begin < row_end || !(signal && signal->n_ranks > 1), "a rendezvous needs a non-empty row range (the kernel runs it)");
     LutMultiArgs M;
     memset(&M, 0, sizeof(M));
-    int rc = vq_fill_peer_sync(signal, &M.sync); if (rc) return rc;
+    int rc = vq_fill_peer_sync(ctx, signal, &M.sync); if (rc) return rc;
     VQ_REQUIRE(M.sync.n == 0 || n_outs > 1, "a rendezvous only makes sense with peer destinations");
     rc = vq_enter(ctx); if (rc) return rc;
     VQ_MARK("CreateBRDFIntegralLUT");

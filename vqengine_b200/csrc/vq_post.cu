@@ -894,7 +894,7 @@ extern "C" int vq_fsr_easu(VqContext* ctx, const uint32_t con[16], int address_m
 // The destination checks every multi-destination post call shares, before the device is touched: 1..8 destinations of exactly the
 // W x H output (`size_msg`, the single call's message, otherwise), none equal to `in` unless the pass may run in place
 // (`alias_msg` == nullptr: the tonemapper), then the row range and the signal as vq_multi_dest_check takes them. Fills `d`.
-static int post_dests_check(VqImage in, const VqImage* outs, int n_outs, int W, int H, const char* size_msg, const char* alias_msg,
+static int post_dests_check(const VqContext* ctx, VqImage in, const VqImage* outs, int n_outs, int W, int H, const char* size_msg, const char* alias_msg,
                             int row_begin, int row_end, const VqPeerSignal* sig, PostDests& d) {
     VQ_REQUIRE(outs, "null destination list");
     VQ_REQUIRE(n_outs >= 1 && n_outs <= 8, "1..8 destinations");
@@ -904,7 +904,7 @@ static int post_dests_check(VqImage in, const VqImage* outs, int n_outs, int W, 
         VQ_REQUIRE(!alias_msg || outs[k].ptr != in.ptr, alias_msg);
     }
     memset(&d, 0, sizeof(d));
-    const int rc = vq_multi_dest_check(outs, n_outs, W, H, 0, row_begin, row_end, sig, d.sync); if (rc) return rc;
+    const int rc = vq_multi_dest_check(ctx, outs, n_outs, W, H, 0, row_begin, row_end, sig, d.sync); if (rc) return rc;
     for (int k = 0; k < n_outs; ++k) d.o[k] = make_view(outs[k]);
     d.n = n_outs; d.w = W; d.h = H; d.rowBegin = row_begin; d.rowEnd = row_end;
     return VQ_OK;
@@ -927,7 +927,7 @@ extern "C" int vq_tonemap_multi_signal(VqContext* ctx, const VqTonemapperParams*
     VQ_REQUIRE(p, "params is null");
     VQ_REQUIRE(vq_image_ok(in), "bad image descriptor");
     PostDests d;
-    int rc = post_dests_check(in, outs, n_outs, in.width, in.height, "tonemap: in/out size mismatch", nullptr, row_begin, row_end,
+    int rc = post_dests_check(ctx, in, outs, n_outs, in.width, in.height, "tonemap: in/out size mismatch", nullptr, row_begin, row_end,
                               signal, d); if (rc) return rc;
     rc = vq_enter(ctx); if (rc) return rc;
     VQ_MARK("TonemapperCS");
@@ -942,7 +942,7 @@ extern "C" int vq_cas_multi_signal(VqContext* ctx, const uint32_t cas_const[8], 
     VQ_REQUIRE(cas_const, "cas_const is null");
     VQ_REQUIRE(vq_image_ok(in), "bad image descriptor");
     PostDests d;
-    int rc = post_dests_check(in, outs, n_outs, in.width, in.height, "cas: sharpen-only path needs equal sizes (FFXCAS_NO_UPSCALING)",
+    int rc = post_dests_check(ctx, in, outs, n_outs, in.width, in.height, "cas: sharpen-only path needs equal sizes (FFXCAS_NO_UPSCALING)",
                               "cas: in-place is not supported", row_begin, row_end, signal, d); if (rc) return rc;
     rc = vq_enter(ctx); if (rc) return rc;
     VQ_MARK("FFX-CAS CS");
@@ -958,7 +958,7 @@ extern "C" int vq_fsr_rcas_multi_signal(VqContext* ctx, const uint32_t rcas_cons
     VQ_REQUIRE(rcas_const, "rcas_const is null");
     VQ_REQUIRE(vq_image_ok(in), "bad image descriptor");
     PostDests d;
-    int rc = post_dests_check(in, outs, n_outs, in.width, in.height, "rcas: in/out size mismatch", "rcas: in-place is not supported",
+    int rc = post_dests_check(ctx, in, outs, n_outs, in.width, in.height, "rcas: in/out size mismatch", "rcas: in-place is not supported",
                               row_begin, row_end, signal, d); if (rc) return rc;
     rc = vq_enter(ctx); if (rc) return rc;
     VQ_MARK("FSR-RCAS CS");
@@ -976,7 +976,7 @@ extern "C" int vq_fsr_easu_multi_signal(VqContext* ctx, const uint32_t con[16], 
     VQ_REQUIRE(address_mode == VQ_ADDRESS_WRAP || address_mode == VQ_ADDRESS_CLAMP, "easu: unknown address mode");
     const int W = outs && n_outs >= 1 ? outs[0].width : 0, H = outs && n_outs >= 1 ? outs[0].height : 0;
     PostDests d;
-    int rc = post_dests_check(in, outs, n_outs, W, H, "every destination must have the size of the first",
+    int rc = post_dests_check(ctx, in, outs, n_outs, W, H, "every destination must have the size of the first",
                               "easu: in-place is not supported", row_begin, row_end, signal, d); if (rc) return rc;
     EasuCon c; memcpy(&c, con, 16);
     const float c0[4] = {c.c0x, c.c0y, c.c0z, c.c0w};
@@ -1300,7 +1300,7 @@ extern "C" int vq_post_process_multi_signal(VqContext* ctx, const VqTonemapperPa
     PostPlan plan;
     int rc = post_process_check(tonemapper, cas_const, easu_const, address_mode, rcas_const, scene_color, W, H, plan); if (rc) return rc;
     PostDests d;
-    rc = post_dests_check(scene_color, outs, n_outs, W, H, "every destination must have the size of the first",
+    rc = post_dests_check(ctx, scene_color, outs, n_outs, W, H, "every destination must have the size of the first",
                           plan.fsr || plan.cas ? "post_process: in-place is not supported with EASU/RCAS or CAS" : nullptr,
                           row_begin, row_end, signal, d); if (rc) return rc;
     rc = vq_enter(ctx); if (rc) return rc;

@@ -209,7 +209,7 @@ extern "C" int vq_forward_lighting_shadowed_multi_signal(VqContext* ctx, const V
     if (gb->emissive.ptr)
         VQ_REQUIRE(vq_image_ok(gb->emissive) && gb->emissive.width == W && gb->emissive.height == H, "bad emissive plane");
     PeerSync sync;
-    rc = vq_multi_dest_check(outs, n_outs, W, H, dst_row_offset, row_begin, row_end, signal, sync); if (rc) return rc;
+    rc = vq_multi_dest_check(ctx, outs, n_outs, W, H, dst_row_offset, row_begin, row_end, signal, sync); if (rc) return rc;
     rc = vq_enter(ctx); if (rc) return rc;
     VQ_MARK("RenderSceneColor");
     return shadowed_passes(ctx, pf, pv, gb, env, *sm, outs, n_outs, dst_row_offset, row_begin, row_end, signal, (cudaStream_t)stream);

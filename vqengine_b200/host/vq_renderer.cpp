@@ -420,6 +420,7 @@ bool VQRendererGroup::Initialize(const std::vector<int>& Devices, uint32_t* cons
     mShadowRecordsSized.assign(mRanks.size(), 0);
     mDisplay.assign(mRanks.size(), VqImage{});
     mEpoch = FirstEpoch;
+    mRendezvousFailed = false;
     return true;
 }
 
@@ -439,6 +440,49 @@ std::vector<VqImage> VQRendererGroup::Targets(int r, const FTexture2D VQRenderer
     return outs;
 }
 
+bool VQRendererGroup::Usable(const char* what) const {
+    if (!mGroup) return GroupFail("VQRendererGroup: not initialized");
+    if (mRendezvousFailed) return GroupFail(std::string(what) + ": a rendezvous failed; Resync() first");
+    return true;
+}
+
+bool VQRendererGroup::SetRendezvousDeadline(uint64_t ns) {
+    if (!mGroup) return GroupFail("VQRendererGroup: not initialized");
+    VQ_TRY(vq_group_set_rendezvous_deadline(mGroup, ns), "vq_group_set_rendezvous_deadline");
+    return true;
+}
+
+bool VQRendererGroup::RendezvousOK() {
+    if (!mGroup) return GroupFail("VQRendererGroup: not initialized");
+    std::string why;
+    for (int r = 0; r < NumRanks(); ++r) {
+        cudaSetDevice(mRanks[r]->Device());
+        VqRendezvousStatus st;
+        if (cudaStreamSynchronize(mStreams[r]) != cudaSuccess) { cudaGetLastError(); return GroupFail("RendezvousOK: device error"); }
+        if (vq_ctx_rendezvous_status(mRanks[r]->mCtx, mStreams[r], &st) != VQ_OK) return Fail("vq_ctx_rendezvous_status");
+        if (!st.failures) continue;
+        why += (why.empty() ? "" : "; ") + std::string("rank ") + std::to_string(r) + ": " + std::to_string(st.failures) +
+               " rendezvous gave up (epochs " + std::to_string(st.first_epoch) + ".." + std::to_string(st.last_epoch) +
+               (st.cancelled ? ", cancelled" : "") + "), missing rank(s)";
+        for (int j = 0; j < 8; ++j)
+            if (st.missing_mask >> j & 1u) why += " " + std::to_string(j);
+    }
+    if (why.empty()) return true;
+    mRendezvousFailed = true;
+    return GroupFail("RendezvousOK: " + why);
+}
+
+bool VQRendererGroup::Resync() {
+    if (!mGroup) return GroupFail("VQRendererGroup: not initialized");
+    const uint32_t e = mEpoch++;
+    for (int r = 0; r < NumRanks(); ++r) {
+        VQ_TRY(vq_ctx_rendezvous_clear(mRanks[r]->mCtx, mStreams[r]), "vq_ctx_rendezvous_clear");
+        VQ_TRY(vq_group_barrier(mGroup, r, e, mStreams[r]), "vq_group_barrier");
+    }
+    mRendezvousFailed = false;
+    return RendezvousOK();
+}
+
 template <class F> bool VQRendererGroup::Phase(uint32_t epoch, F issue) {
     for (int r = 0; r < NumRanks(); ++r) {
         VqPeerSignal sig;
@@ -455,7 +499,7 @@ template <class F> bool VQRendererGroup::Phase(uint32_t epoch, F issue) {
 }
 
 bool VQRendererGroup::LoadDefaultResources() {
-    if (!mGroup) return GroupFail("VQRendererGroup: not initialized");
+    if (!Usable("LoadDefaultResources")) return false;
     for (auto& r : mRanks) {
         cudaSetDevice(r->Device());
         if (!r->mBRDFLUT.Create(1024, 1024, 8)) return false;    // Renderer.cpp:1026-1032
@@ -471,7 +515,7 @@ bool VQRendererGroup::LoadDefaultResources() {
     });
     bool synced = true;
     for (int r = 0; r < n; ++r) synced = cudaStreamSynchronize(mStreams[r]) == cudaSuccess && synced;
-    return ok && (synced || GroupFail("LoadDefaultResources: device error"));
+    return ok && (synced || GroupFail("LoadDefaultResources: device error")) && RendezvousOK();
 }
 
 bool VQRendererGroup::OnWindowSizeChanged(int rw, int rh, int dw, int dh) {
@@ -492,7 +536,7 @@ bool VQRendererGroup::OnWindowSizeChanged(int rw, int rh, int dw, int dh) {
 }
 
 bool VQRendererGroup::PreFilterEnvironmentMap(const PerRank<FEnvironmentMapRenderingResources*>& envs, float step) {
-    if (!mGroup) return GroupFail("VQRendererGroup: not initialized");
+    if (!Usable("PreFilterEnvironmentMap")) return false;
     const int n = NumRanks();
     if ((int)envs.size() != n) return GroupFail("PreFilterEnvironmentMap: one environment per rank");
     for (int r = 0; r < n; ++r) {
@@ -543,6 +587,7 @@ bool VQRendererGroup::PreFilterEnvironmentMap(const PerRank<FEnvironmentMapRende
     bool synced = true;
     for (int r = 0; r < n; ++r) { cudaSetDevice(mRanks[r]->Device()); synced = cudaStreamSynchronize(mStreams[r]) == cudaSuccess && synced; }
     if (!synced) { for (auto& m : mPrepared) m = VqEnvironmentMaps{}; return GroupFail("PreFilterEnvironmentMap: device error"); }
+    if (ok && !RendezvousOK()) { for (auto& m : mPrepared) m = VqEnvironmentMaps{}; return false; }
     return ok;
 }
 
@@ -582,7 +627,7 @@ struct VQRendererGroup::FSceneCall {
 };
 
 bool VQRendererGroup::RenderScene(const FSceneCall& c) {
-    if (!mGroup) return GroupFail("VQRendererGroup: not initialized");
+    if (!Usable("RenderSceneColor")) return false;
     const int n = NumRanks();
     const bool gbuf = c.GBuffers != nullptr;
     if (!mRanks[0]->mSceneColor.mem.ptr) return GroupFail("RenderSceneColor: OnWindowSizeChanged first");
@@ -692,7 +737,7 @@ bool VQRendererGroup::RenderSceneColorFromMaterials(const FSceneView& SceneView,
 }
 
 bool VQRendererGroup::ApplyReflections(const PerRank<VqImage>& ReflectionRadiance, const PerRank<VqImage>* BoundingVolumes) {
-    if (!mGroup) return GroupFail("VQRendererGroup: not initialized");
+    if (!Usable("ApplyReflections")) return false;
     const int n = NumRanks();
     if (!mRanks[0]->mSceneColor.mem.ptr) return GroupFail("ApplyReflections: OnWindowSizeChanged first");
     if ((int)ReflectionRadiance.size() != n || (BoundingVolumes && (int)BoundingVolumes->size() != n))
@@ -710,7 +755,7 @@ bool VQRendererGroup::ApplyReflections(const PerRank<VqImage>& ReflectionRadianc
 }
 
 const VqImage* VQRendererGroup::RenderPostProcess(const FPostProcessParameters& PPParams, bool /*bHDR*/) {
-    if (!mGroup) { GroupFail("VQRendererGroup: not initialized"); return nullptr; }
+    if (!Usable("RenderPostProcess")) return nullptr;
     if (PPParams.bEnableGaussianBlur) { GroupFail("RenderPostProcess: the Gaussian blur has no band form in a group"); return nullptr; }
     if (!mRanks[0]->mSceneColor.mem.ptr) { GroupFail("RenderPostProcess: OnWindowSizeChanged first"); return nullptr; }
     const int n = NumRanks();

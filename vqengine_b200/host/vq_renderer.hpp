@@ -338,12 +338,26 @@ public:
     // is refused.
     const VqImage* RenderPostProcess(const FPostProcessParameters& PPParams, bool bHDR);
 
+    // ---- a step whose peer does not come back (vqcuda_rendezvous.h, DESIGN.md §6) ----
+    // Registers a rendezvous deadline of Ns nanoseconds on every rank's context (1 ns..20 s; without one a wait that is never met
+    // traps after 20 s). A rank whose wait gives up then ends its call normally and records the failure in its context's status.
+    bool SetRendezvousDeadline(uint64_t Ns);
+    // BLOCKS: synchronises every rank's stream and reads every rank's status. False, with LastError() naming each rank that saw a
+    // failure and the ranks it missed, when a wait gave up since the last Resync(). LoadDefaultResources and
+    // PreFilterEnvironmentMap check this themselves and return false. After a failure every signalled method refuses (returns
+    // false, enqueues nothing) until Resync() succeeds: a late peer may still be storing an earlier step into a rank's targets.
+    bool RendezvousOK();
+    // BLOCKS: every rank clears its status and meets its peers at a fresh epoch (vq_group_barrier), then the statuses are read.
+    // True once every rank met every peer: every store of the earlier steps, a late peer's included, has landed.
+    bool Resync();
+
 private:
     struct FSceneCall;
     bool RenderScene(const FSceneCall& call);
     // one signalled phase: issue(r) on every rank in order; if a rank refuses, the ranks from it on arrive at `epoch` in their
     // peers' flag arrays (vq_group_arrive), so that the ranks already enqueued finish instead of waiting for them
     template <class F> bool Phase(uint32_t epoch, F issue);
+    bool Usable(const char* what) const;                        // initialized, and no rendezvous failure awaits a Resync()
     std::vector<VqImage> Targets(int r, const FTexture2D VQRenderer::* member) const;   // rank r's destinations in its rank order
     bool Prepared(const PerRank<const FEnvironmentMapRenderingResources*>& envs) const;
 
@@ -353,6 +367,7 @@ private:
     std::vector<VqImage> mDisplay;
     VqGroup* mGroup = nullptr;
     uint32_t mEpoch = 1;
+    bool mRendezvousFailed = false;                            // a wait gave up; the signalled methods refuse until Resync()
     std::vector<char> mShadowRecordsSized;                     // per rank: a PCF test has sized the records at this size (rule 3, DESIGN §6)
 };
 
