@@ -339,6 +339,8 @@ VQ_API int vq_fsr_easu(VqContext* ctx, const uint32_t easu_const[16], int addres
 /* ------------------------------------------------------------------------------------------
  * K9  FSR1 RCAS.  Replaces SceneRendering.cpp:2735-2781 + FSR_RCAS_CSMain (AMDFidelityFX.hlsl:335-376)
  *     -> FsrRcasF (ffx_fsr1.h:684-769). rcas_const = FFSR1_RCAS::RCASConstantBlock (4 words).
+ *     Subnormal channels: the hitMin reciprocal reads a subnormal 4*mx4 as 0 (rcp.approx.ftz). Where it does, the result is
+ *     FsrRcasF of the input with that channel's subnormals flushed to zeros of their sign (D3D11 allows flushing); DESIGN §5.
  * ------------------------------------------------------------------------------------------ */
 VQ_API int vq_fsr_rcas(VqContext* ctx, const uint32_t rcas_const[4], VqImage in, VqImage out, void* stream);
 

@@ -5,10 +5,12 @@
 
 extern "C" {
 
-// con0 = (scale x, scale y, bias x, bias y); returns the verdict (0 = accepted) and, in out3, {path, ncx, ncy}
-int hostcheck_easu_check(const float con0[4], int in_w, int in_h, int out_w, int out_h, int* out3) {
+// con0 = (scale x, scale y, bias x, bias y); `fused` selects the up path's tiling: 0 = easu_up_kernel's (EASU_UP_TILE, what
+// vq_fsr_easu checks), 1 = post_fsr_up_kernel's (FUSED_UP_TILE, what vq_post_process checks). Returns the verdict (0 = accepted)
+// and, in out3, {path, ncx, ncy}
+int hostcheck_easu_check(const float con0[4], int in_w, int in_h, int out_w, int out_h, int fused, int* out3) {
     int ncx = 0, ncy = 0;
-    const int v = vqeasu::check(con0, in_w, in_h, out_w, out_h, &ncx, &ncy);
+    const int v = vqeasu::check(con0, in_w, in_h, out_w, out_h, &ncx, &ncy, fused ? vqeasu::FUSED_UP_TILE : vqeasu::EASU_UP_TILE);
     out3[0] = vqeasu::path(con0, in_w, in_h, out_w, out_h);
     out3[1] = ncx;
     out3[2] = ncy;

@@ -1,6 +1,7 @@
 """CPU (-m "not gpu"): the post chain's float64 restatements (tests/post_ref.py) against the oracle over the domain images of
 tests/post_domain.py, and the EASU constant check (vqengine_b200/csrc/vq_easu_check.cuh) built for the host and swept over
-every constant FsrEasuCon builds for viewport <= input <= 8192 and output <= 16384."""
+every constant FsrEasuCon builds for viewport <= input <= 8192 and output <= 16384, under both up-path tilings: vq_fsr_easu's
+(easu_up_kernel) and vq_post_process's (post_fsr_up_kernel)."""
 import ctypes as C
 import os
 import subprocess
@@ -36,15 +37,16 @@ def easu_host(tmp_path_factory):
     subprocess.check_call(["g++", "-O2", "-std=c++17", "-fPIC", "-ffp-contract=off", "-fno-fast-math", "-shared", "-o", str(out),
                            os.path.join(ROOT, "tests", "host_check", "easu_check_host.cpp")])
     lib = C.CDLL(str(out))
-    lib.hostcheck_easu_check.argtypes = [C.POINTER(C.c_float), C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int)]
+    lib.hostcheck_easu_check.argtypes = [C.POINTER(C.c_float), C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int)]
     lib.hostcheck_easu_f.argtypes = [C.c_float, C.c_float, C.c_int, C.POINTER(C.c_int)]
     return lib
 
 
-def easu_check(lib, con0, iw, ih, ow, oh):
+def easu_check(lib, con0, iw, ih, ow, oh, fused=False):
+    """the check vq_fsr_easu makes, or with `fused` the one vq_post_process makes: (verdict, (path, ncx, ncy))"""
     c = (C.c_float * 4)(*[float(v) for v in con0[:4]])
     o = (C.c_int * 3)()
-    v = lib.hostcheck_easu_check(c, iw, ih, ow, oh, o)
+    v = lib.hostcheck_easu_check(c, iw, ih, ow, oh, int(fused), o)
     return v, tuple(o)
 
 
@@ -134,34 +136,66 @@ def _fsr_pairs():
     return out
 
 
-def test_every_fsr_easu_con_is_accepted(easu_host):
+# post_fsr_up_kernel's tiling (vq_post.cu): 30 x 14 display tiles, EASU on each widened by RCAS's 1-pixel ring, clipped to the
+# display, and 32 x 16 candidate 'f' texels. Written out here from the kernel, so that a FUSED_UP_TILE that stops describing
+# the kernel fails the comparisons below.
+FUSED_TILE, FUSED_RING, FUSED_CAP = (30, 14), 1, (32, 16)
+
+
+def sweep_fsr_easu_cons(lib, fused, cap):
+    """asserts that no FsrEasuCon upscale is refused and that every up-path footprint fits `cap`; returns the number of up-path
+    constants and the largest footprint (ncx, ncy)"""
     import vqengine_b200 as vq
-    up = worst = 0
+    up = worst_x = worst_y = 0
     for (vw, vh), (iw, ih), (ow, oh) in _fsr_pairs():
         c0 = con0_of(vq.fsr_easu_con(vw, vh, iw, ih, ow, oh))
-        v, (path, ncx, ncy) = easu_check(easu_host, c0, iw, ih, ow, oh)
+        v, (path, ncx, ncy) = easu_check(lib, c0, iw, ih, ow, oh, fused)
         assert v == 0, ((vw, vh), (iw, ih), (ow, oh), v)
         if path == 1:
             up += 1
-            assert 1 <= ncx <= 32 and 1 <= ncy <= 8
-            worst = max(worst, ncx)
-    assert up > 50 and worst == 32                           # ratio 1 fills the 32-wide tile exactly
+            assert 1 <= ncx <= cap[0] and 1 <= ncy <= cap[1], ((vw, vh), (iw, ih), (ow, oh), ncx, ncy)
+            worst_x, worst_y = max(worst_x, ncx), max(worst_y, ncy)
+    return up, (worst_x, worst_y)
+
+
+def test_every_fsr_easu_con_is_accepted(easu_host):
+    """vq_fsr_easu's check (easu_up_kernel's 32 x 8 tiles): ratio 1 fills the 32-wide tile exactly"""
+    up, worst = sweep_fsr_easu_cons(easu_host, False, (32, 8))
+    assert up > 50 and worst == (32, 8)
+
+
+def test_every_fsr_easu_con_runs_fused(easu_host):
+    """vq_post_process's check (post_fsr_up_kernel's 30 x 14 tiles and ring): no refusal, and the footprint reaches the
+    32 x 16 candidate capacity on both axes"""
+    up, worst = sweep_fsr_easu_cons(easu_host, True, FUSED_CAP)
+    assert up > 50 and worst == FUSED_CAP
+
+
+def brute_force_candidates(f, tile, ring):
+    """the largest span of 'f' texels (max - min + 1, what a tile stages) over tiles of `tile` outputs at multiples of `tile`,
+    each widened by `ring` outputs on both sides and clipped to [0, n_out): taken from every output's 'f'"""
+    n_out = len(f)
+    return max(int(np.ptp(f[max(o0 - ring, 0):min(o0 + tile + ring, n_out)])) + 1 for o0 in range(0, n_out, tile))
 
 
 @pytest.mark.parametrize("scale,bias,n_out", [(0.5, -0.25, 4097), (0.77, -0.115, 3000), (0.99, -0.005, 16384), (1.0, 0.0, 999),
                                               (1.0, -0.5, 8192), (3.0, 1.0, 700), (-0.5, 100.0, 300)])
 def test_extent_endpoints_bound_every_pixel(easu_host, scale, bias, n_out):
-    """easu_pos is monotone, so its two ends bound every output's 'f'; the tile footprint equals a brute-force count"""
+    """easu_pos is monotone, so its two ends bound every output's 'f'; the footprint the check reports under each kernel's
+    tiling equals a brute-force count of that tiling"""
     f = (C.c_int * n_out)()
     easu_host.hostcheck_easu_f(scale, bias, n_out, f)
     f = np.array(f)
     assert f.min() == min(f[0], f[-1]) and f.max() == max(f[0], f[-1])
     assert (np.diff(f) * np.sign(scale) >= 0).all()
     if 0 < scale <= 1:
-        n = max(int(f[min(o + 31, n_out - 1)] - f[o] + 1) for o in range(0, n_out, 32))
         iw = int(f.max()) + 3
         v, (path, ncx, ncy) = easu_check(easu_host, [scale, scale, bias, bias], iw, iw, n_out, n_out)
-        assert v == 0 and path == 1 and ncx == n
+        assert v == 0 and path == 1 and ncx == brute_force_candidates(f, 32, 0) and ncy == brute_force_candidates(f, 8, 0)
+        v, (path, ncx, ncy) = easu_check(easu_host, [scale, scale, bias, bias], iw, iw, n_out, n_out, fused=True)
+        want = tuple(brute_force_candidates(f, t, FUSED_RING) for t in FUSED_TILE)
+        assert path == 1 and (ncx, ncy) == want, ((ncx, ncy), want)
+        assert v == (0 if want[0] <= FUSED_CAP[0] and want[1] <= FUSED_CAP[1] else 3)
 
 
 @pytest.mark.parametrize("case", ["stale_after_resize", "viewport_larger", "nan", "inf", "neg_inf", "huge_bias", "far_negative"])

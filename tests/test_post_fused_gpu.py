@@ -83,8 +83,9 @@ def assert_same(got, want, what):
     assert np.array_equal(g, w), (what, int((g != w).any(-1).sum()), np.argwhere((g != w).any(-1))[:4].tolist())
 
 
-def fsr_consts(ih, iw, oh, ow, stops=0.2):
-    return vq.fsr_easu_con(iw, ih, iw, ih, ow, oh), vq.fsr_rcas_con(stops)
+def fsr_consts(ih, iw, oh, ow, stops=0.2, vp=None):
+    vh, vw = vp or (ih, iw)
+    return vq.fsr_easu_con(vw, vh, iw, ih, ow, oh), vq.fsr_rcas_con(stops)
 
 
 def check_fsr(ctx, src, oh, ow, mode=vq.VQ_ADDRESS_WRAP, tm=None, stops=0.2):
@@ -214,13 +215,17 @@ def test_two_streams_of_one_context(ctx):
 
 
 # ---- multi-destination form ----------------------------------------------------------------------------------------------------
+# (case, input h, w, display h, w) and, for FsrEasuCon with a viewport smaller than the input, VIEWPORTS[case] = (h, w): the up path
+# with viewport < input, at ratio 0.99, at scale 0.5 (2x constants on an input that is not half the display) and on a 2 x 7 input
 BRANCHES = [("fsr 2x", 23, 37, 46, 74), ("fsr 2x tall", 61, 20, 122, 40), ("fsr preset", 41, 73, 54, 95), ("fsr 1:1", 37, 61, 37, 61),
-            ("cas", 37, 61, None, None), ("tonemap", 37, 61, None, None)]
+            ("fsr viewport < input", 40, 64, 60, 96), ("fsr 0.99", 50, 63, 51, 64), ("fsr scale 0.5", 19, 40, 34, 62),
+            ("fsr 2x7 to 5x13", 7, 2, 13, 5), ("cas", 37, 61, None, None), ("tonemap", 37, 61, None, None)]
+VIEWPORTS = {"fsr viewport < input": (30, 48), "fsr scale 0.5": (17, 31)}
 
 
 def branch_consts(case, ih, iw, oh, ow):
     if case.startswith("fsr"):
-        easu, rcas = fsr_consts(ih, iw, oh, ow)
+        easu, rcas = fsr_consts(ih, iw, oh, ow, vp=VIEWPORTS.get(case))
         return dict(easu=easu, rcas=rcas), (oh, ow)
     if case == "cas":
         return dict(cas=vq.cas_setup(0.6, iw, ih, iw, ih)), (ih, iw)
@@ -254,19 +259,26 @@ def test_multi_equals_single(ctx, mode, n_dests, case, ih, iw, oh, ow):
 
 WORLDS = [("fsr wrap", 270, 480, 2.0, vq.VQ_ADDRESS_WRAP, False), ("fsr clamp", 270, 480, 2.0, vq.VQ_ADDRESS_CLAMP, False),
           ("fsr + cas", 270, 480, 2.0, vq.VQ_ADDRESS_WRAP, True), ("fsr preset ragged", 41, 73, 1 / 0.77, vq.VQ_ADDRESS_WRAP, False),
-          ("fsr 2x ragged clamp", 23, 37, 2.0, vq.VQ_ADDRESS_CLAMP, False), ("cas", 270, 480, None, None, True),
-          ("cas ragged", 37, 61, None, None, True), ("tonemap", 270, 480, None, None, False), ("tonemap ragged", 37, 61, None, None, False)]
+          ("fsr 2x ragged clamp", 23, 37, 2.0, vq.VQ_ADDRESS_CLAMP, False),
+          ("fsr viewport < input", 40, 64, (60, 96), vq.VQ_ADDRESS_WRAP, False), ("fsr 0.99", 69, 99, (70, 100), vq.VQ_ADDRESS_CLAMP, False),
+          ("fsr scale 0.5", 19, 40, (34, 62), vq.VQ_ADDRESS_WRAP, False), ("fsr 2x7 to 5x13", 7, 2, (13, 5), vq.VQ_ADDRESS_WRAP, False),
+          ("cas", 270, 480, None, None, True), ("cas ragged", 37, 61, None, None, True), ("tonemap", 270, 480, None, None, False),
+          ("tonemap ragged", 37, 61, None, None, False)]
 
 
 @pytest.mark.parametrize("n", [1, 2, 3, 8])
 @pytest.mark.parametrize("case,ih,iw,scale,mode,cas", WORLDS, ids=[w[0] for w in WORLDS])
 def test_simulated_world_assembles_the_single_gpu_chain(ctx, n, case, ih, iw, scale, mode, cas):
-    """every rank on this GPU, its peers' display frames as local destinations, ONE fused launch per rank into NaN-filled frames"""
+    """every rank on this GPU, its peers' display frames as local destinations, ONE fused launch per rank into NaN-filled frames;
+    `scale` is the display's ratio to the input or its (h, w)"""
     src = hdr(ih, iw, 4)
     tm = synth.default_tonemapper()
     if scale is not None:
-        oh, ow = (2 * ih, 2 * iw) if scale == 2.0 else (round(ih * scale), round(iw * scale))
-        easu, rcas = fsr_consts(ih, iw, oh, ow)
+        if isinstance(scale, tuple):
+            oh, ow = scale
+        else:
+            oh, ow = (2 * ih, 2 * iw) if scale == 2.0 else (round(ih * scale), round(iw * scale))
+        easu, rcas = fsr_consts(ih, iw, oh, ow, vp=VIEWPORTS.get(case))
     else:
         oh, ow, easu, rcas = ih, iw, None, None
     cas_con = vq.cas_setup(0.5, iw, ih, iw, ih) if cas else None
