@@ -302,6 +302,7 @@ VQ_API int vq_brdf_integration_lut(VqContext* ctx, VqImage out_rg, int num_sampl
 VQ_API int vq_gaussian_blur_x(VqContext* ctx, const VqBlurParams* params, VqImage in, VqImage out, void* stream);
 VQ_API int vq_gaussian_blur_y(VqContext* ctx, const VqBlurParams* params, VqImage in, VqImage out, void* stream);
 /* A whole one-mip cube, X then Y, in one launch: vq_gaussian_blur_cube (vqcuda_prefilter_multi.h). */
+/* X then Y in one launch, and its band form for a multi-GPU frame: vq_gaussian_blur, vq_gaussian_blur_multi_signal (vqcuda_blur.h). */
 
 /* ------------------------------------------------------------------------------------------
  * K6  Tonemapper.  Replaces the dispatch at SceneRendering.cpp:2640-2656 + CSMain (Tonemapper.hlsl:110-151).
@@ -695,5 +696,8 @@ VQ_API int vq_forward_lighting_host(VqContext* ctx,
 
 /* The environment prefilter across GPUs: the band forms of K2 and K4 and the one-launch cube blur. */
 #include "vqcuda_prefilter_multi.h"
+
+/* The Gaussian blur of the post chain in one launch, and its band form. */
+#include "vqcuda_blur.h"
 
 #endif /* VQCUDA_H */

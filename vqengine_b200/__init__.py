@@ -42,6 +42,8 @@ ABI_SYMBOLS = [
 ]
 # every symbol include/vqcuda_prefilter_multi.h declares (the environment prefilter across GPUs; vqcuda.h includes that header)
 PREFILTER_MULTI_SYMBOLS = ["vq_diffuse_irradiance_multi_signal", "vq_brdf_integration_lut_multi_signal", "vq_gaussian_blur_cube"]
+# every symbol include/vqcuda_blur.h declares (the one-launch blur and its band form; vqcuda.h includes that header)
+BLUR_SYMBOLS = ["vq_gaussian_blur", "vq_gaussian_blur_multi_signal"]
 # every symbol include/vqcuda_group.h declares (the device group of a multi-GPU world in one process)
 GROUP_SYMBOLS = ["vq_group_create", "vq_group_destroy", "vq_group_rank_order", "vq_group_signal", "vq_group_arrive", "vq_band_rows",
                  "vq_specular_rank_ranges", "vq_group_set_rendezvous_deadline", "vq_group_cancel", "vq_group_barrier"]
@@ -101,6 +103,8 @@ def _load() -> C.CDLL:
     lib.vq_gaussian_blur_cube.argtypes = [vp, Cubemap, Cubemap, vp]
     lib.vq_gaussian_blur_x.argtypes = [vp, P(BlurParams), Image, Image, vp]
     lib.vq_gaussian_blur_y.argtypes = [vp, P(BlurParams), Image, Image, vp]
+    lib.vq_gaussian_blur.argtypes = [vp, P(BlurParams), Image, Image, vp]
+    lib.vq_gaussian_blur_multi_signal.argtypes = [vp, P(BlurParams), Image, P(Image), C.c_int, C.c_int, C.c_int, P(PeerSignal), vp]
     lib.vq_tonemap.argtypes = [vp, P(TonemapperParams), Image, Image, vp]
     lib.vq_cas.argtypes = [vp, P(u32), Image, Image, vp]
     lib.vq_fsr_easu.argtypes = [vp, P(u32), C.c_int, Image, Image, vp]
@@ -705,6 +709,10 @@ class Context:
         fn = lib.vq_gaussian_blur_y if vertical else lib.vq_gaussian_blur_x
         _check(fn(self._h, C.byref(p), image_of(src), image_of(dst), _stream_ptr(stream)))
 
+    def gaussian_blur2d(self, params: BlurParams, src, dst, stream=None):
+        """both blur passes, X then Y, in one launch with no intermediate image (vq_gaussian_blur)"""
+        _check(lib.vq_gaussian_blur(self._h, C.byref(params), image_of(src), image_of(dst), _stream_ptr(stream)))
+
     def tonemap(self, params: TonemapperParams, src, dst, stream=None):
         _check(lib.vq_tonemap(self._h, C.byref(params), image_of(src), image_of(dst), _stream_ptr(stream)))
 
@@ -724,6 +732,11 @@ class Context:
         re = (out_images[0].height if out_images else 0) if row_end is None else row_end
         _check(fn(self._h, *args, image_of(src), arr, len(out_images), row_begin, re,
                   C.byref(signal) if signal is not None else None, _stream_ptr(stream)))
+
+    def gaussian_blur_multi(self, params: BlurParams, src, out_images, row_begin=0, row_end=None, stream=None, signal=None):
+        """gaussian_blur2d on rows [row_begin, row_end) into every destination (row_end default: params.iImageSizeY)"""
+        self._post_multi(lib.vq_gaussian_blur_multi_signal, (C.byref(params),), src, out_images, row_begin,
+                         params.iImageSizeY if row_end is None else row_end, stream, signal)
 
     def tonemap_multi(self, params: TonemapperParams, src, out_images, row_begin=0, row_end=None, stream=None, signal=None):
         self._post_multi(lib.vq_tonemap_multi_signal, (C.byref(params),), src, out_images, row_begin, row_end, stream, signal)

@@ -268,14 +268,21 @@ __global__ void __launch_bounds__(BYM_T) blur_y_kernel(ImgV in, ImgV out, int si
     }
 }
 
-static int blur_common(VqContext* ctx, const VqBlurParams* p, VqImage in, VqImage out, void* stream, bool vertical) {
-    int rc = vq_enter(ctx); if (rc) return rc;
+// The argument checks of every planar blur call (vq_gaussian_blur_x / _y, vq_gaussian_blur, vq_gaussian_blur_multi_signal's
+// source against each destination)
+static int blur_check(const VqBlurParams* p, VqImage in, VqImage out) {
     VQ_REQUIRE(p, "params is null");
     VQ_REQUIRE(vq_image_ok(in) && vq_image_ok(out), "bad image descriptor");
     VQ_REQUIRE(p->iImageSizeX > 0 && p->iImageSizeY > 0, "blur: image size must be positive");
     VQ_REQUIRE(p->iImageSizeX <= in.width && p->iImageSizeY <= in.height &&
                p->iImageSizeX <= out.width && p->iImageSizeY <= out.height, "blur: iImageSize exceeds the images");
     VQ_REQUIRE(in.ptr != out.ptr, "blur: in-place is not supported (the engine ping-pongs too)");
+    return VQ_OK;
+}
+
+static int blur_common(VqContext* ctx, const VqBlurParams* p, VqImage in, VqImage out, void* stream, bool vertical) {
+    int rc = vq_enter(ctx); if (rc) return rc;
+    rc = blur_check(p, in, out); if (rc) return rc;
     const ImgV vi = make_view(in), vo = make_view(out);
     cudaStream_t s = (cudaStream_t)stream;
     if (!vertical) {
@@ -289,6 +296,100 @@ static int blur_common(VqContext* ctx, const VqBlurParams* p, VqImage in, VqImag
 }
 extern "C" int vq_gaussian_blur_x(VqContext* ctx, const VqBlurParams* p, VqImage in, VqImage out, void* stream) { VQ_MARK("BlurX"); return blur_common(ctx, p, in, out, stream, false); }
 extern "C" int vq_gaussian_blur_y(VqContext* ctx, const VqBlurParams* p, VqImage in, VqImage out, void* stream) { VQ_MARK("BlurY"); return blur_common(ctx, p, in, out, stream, true); }
+
+// X then Y in one launch (vq_gaussian_blur, and its band form vq_gaussian_blur_multi_signal as the MULTI instantiation, launched
+// over the tile rows that meet the band). A CTA owns a B2_TW x B2_TH output tile. It runs the X pass on the tile's columns for
+// the B2_TH + 20 rows its Y pass reads (the 10-row halo above and below is recomputed, never read back), keeps those results as
+// fp32 RGB planes in shared memory, and then runs the Y pass from there. The X pass stages 16 clamped input rows at a time in
+// planar shared memory and gives each thread 4 adjacent pixels from a 28-value window, as blur_x_kernel does; the next 16 rows'
+// loads are in flight while a chunk is filtered. The Y pass gives each thread 4 vertically adjacent pixels of one column from 24
+// X rows. Both passes are gauss21 / gauss21_3 on the clamped samples of blur_x_kernel / blur_y_kernel (GaussianBlur.hlsl:144,
+// 180) and the X results are the fp32 values blur_x_kernel stores, so every pixel equals vq_gaussian_blur_x ->
+// vq_gaussian_blur_y bit for bit, with no intermediate image. The shape against a CTA walking down a column strip: DESIGN.md §9.
+constexpr int B2_T = 256;
+constexpr int B2_TW = 64, B2_TH = 64;                      // output tile
+constexpr int B2_XR = B2_TH + 20;                          // X rows per tile: the tile's rows and the 10-row halo each side
+constexpr int B2_SW = B2_TW + 24;                          // staged input columns [x0-12, x0+B2_TW+12), as blur_x_kernel's BX_SM
+constexpr int B2_CR = B2_T / (B2_TW / 4);                  // X rows per staged chunk (16 threads of 4 pixels per row)
+constexpr int B2_NC = (B2_XR + B2_CR - 1) / B2_CR;         // chunks per tile
+constexpr int B2_LD = (B2_CR * B2_SW + B2_T - 1) / B2_T;   // float4 loads per thread per chunk
+constexpr int B2_YR = 4;                                   // Y pass: vertically adjacent pixels per thread per step
+static_assert(B2_TW % 4 == 0 && B2_T % B2_TW == 0 && B2_TH % (B2_YR * (B2_T / B2_TW)) == 0, "tile shape");
+constexpr size_t B2_SMEM = sizeof(float) * 3 * ((size_t)B2_CR * B2_SW + (size_t)B2_XR * B2_TW);
+
+template <bool MULTI = false>
+__global__ void __launch_bounds__(B2_T, 2) blur2d_kernel(ImgV in, PostOut<MULTI> out, int sizeX, int sizeY) {
+    extern __shared__ __align__(16) float b2_sm[];
+    float (*stg)[3][B2_SW] = reinterpret_cast<float (*)[3][B2_SW]>(b2_sm);                     // [B2_CR][3][B2_SW] input
+    float (*xs)[B2_XR][B2_TW] = reinterpret_cast<float (*)[B2_XR][B2_TW]>(b2_sm + 3 * B2_CR * B2_SW);   // [3][B2_XR][B2_TW]
+    const int t = threadIdx.x;
+    const int x0 = blockIdx.x * B2_TW, y0 = tile_row(out) * B2_TH;
+    float4 pre[B2_LD];
+    auto load_chunk = [&](int c) {
+#pragma unroll
+        for (int q = 0; q < B2_LD; ++q) {
+            const int i = t + q * B2_T, r = i / B2_SW, xr = c * B2_CR + r;
+            if (i < B2_CR * B2_SW && xr < B2_XR) {
+                const int sy = min(max(y0 - 10 + xr, 0), sizeY - 1);                    // GaussianBlur.hlsl:180
+                const int sx = min(max(x0 - 12 + (i - r * B2_SW), 0), sizeX - 1);       // GaussianBlur.hlsl:144
+                pre[q] = __ldg(in.row(sy) + sx);
+            }
+        }
+    };
+    load_chunk(0);
+    for (int c = 0; c < B2_NC; ++c) {
+#pragma unroll
+        for (int q = 0; q < B2_LD; ++q) {
+            const int i = t + q * B2_T, r = i / B2_SW, col = i - r * B2_SW;
+            if (i < B2_CR * B2_SW && c * B2_CR + r < B2_XR) { stg[r][0][col] = pre[q].x; stg[r][1][col] = pre[q].y; stg[r][2][col] = pre[q].z; }
+        }
+        __syncthreads();
+        if (c + 1 < B2_NC) load_chunk(c + 1);                                           // in flight while this chunk is filtered
+        const int r = t / (B2_TW / 4), l = t % (B2_TW / 4), xr = c * B2_CR + r;
+        if (xr < B2_XR) {
+#pragma unroll
+            for (int ch = 0; ch < 3; ++ch) {
+                float win[28];                                                           // staged 4l .. 4l+27 == x-12 .. x+15
+                const float4* p = reinterpret_cast<const float4*>(&stg[r][ch][4 * l]);
+#pragma unroll
+                for (int q = 0; q < 7; ++q) { const float4 v = p[q]; win[4 * q] = v.x; win[4 * q + 1] = v.y; win[4 * q + 2] = v.z; win[4 * q + 3] = v.w; }
+                float a[4];
+#pragma unroll
+                for (int j = 0; j < 4; ++j) a[j] = gauss21([&](int k) { return win[j + 2 + k]; });   // tap x+j-10+k
+                *reinterpret_cast<float4*>(&xs[ch][xr][4 * l]) = make_float4(a[0], a[1], a[2], a[3]);
+            }
+        }
+        __syncthreads();                                                                 // stg free; after the last chunk xs is whole
+    }
+    const int cx = t % B2_TW, x = x0 + cx;
+    for (int ly = (t / B2_TW) * B2_YR; ly < B2_TH && y0 + ly < sizeY; ly += B2_YR * (B2_T / B2_TW)) {
+        float3 w[B2_YR + 20];                                                            // X rows y0+ly-10 .. y0+ly+B2_YR+9
+#pragma unroll
+        for (int k = 0; k < B2_YR + 20; ++k) w[k] = f3(xs[0][ly + k][cx], xs[1][ly + k][cx], xs[2][ly + k][cx]);
+#pragma unroll
+        for (int j = 0; j < B2_YR; ++j) {
+            const float3 a = gauss21_3([&](int k) { return w[j + k]; });
+            if (x < sizeX && y0 + ly + j < sizeY) store_px(out, x, y0 + ly + j, make_float4(a.x, a.y, a.z, 1.0f));
+        }
+    }
+    post_retire(out);
+}
+
+template <bool MULTI>
+static int blur2d_launch(dim3 grid, ImgV vi, const PostOut<MULTI>& vo, int sizeX, int sizeY, cudaStream_t s) {
+    VQ_CUDA_OK(cudaFuncSetAttribute(blur2d_kernel<MULTI>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)B2_SMEM));
+    blur2d_kernel<MULTI><<<grid, B2_T, B2_SMEM, s>>>(vi, vo, sizeX, sizeY);
+    return vq_check_launch(MULTI ? "gaussian_blur_multi" : "gaussian_blur");
+}
+
+extern "C" int vq_gaussian_blur(VqContext* ctx, const VqBlurParams* p, VqImage in, VqImage out, void* stream) {
+    int rc = blur_check(p, in, out); if (rc) return rc;
+    rc = vq_enter(ctx); if (rc) return rc;
+    VQ_MARK("Blur");
+    const dim3 grid((p->iImageSizeX + B2_TW - 1) / B2_TW, (p->iImageSizeY + B2_TH - 1) / B2_TH);
+    return blur2d_launch<false>(grid, make_view(in), make_view(out), p->iImageSizeX, p->iImageSizeY, (cudaStream_t)stream);
+}
+
 
 // All six faces of a one-mip cube, X then Y, in one launch: a CTA per face. The X pass reads the face from global memory and keeps
 // its result (RGB planes) in shared memory; after a barrier the Y pass reads those planes and stores the face. Both passes use the
@@ -1009,6 +1110,23 @@ extern "C" int vq_fsr_easu_multi_signal(VqContext* ctx, const uint32_t con[16], 
         else      easu_kernel<VQ_ADDRESS_CLAMP, true><<<grid, dim3(ST_BX, ST_BY), 0, st>>>(vi, d, c);
     }
     return vq_check_launch("fsr_easu_multi");
+}
+
+extern "C" int vq_gaussian_blur_multi_signal(VqContext* ctx, const VqBlurParams* p, VqImage in, const VqImage* outs, int n_outs,
+                                             int row_begin, int row_end, const VqPeerSignal* signal, void* stream) {
+    VQ_REQUIRE(outs, "null destination list");
+    VQ_REQUIRE(n_outs >= 1 && n_outs <= 8, "1..8 destinations");
+    for (int k = 0; k < n_outs; ++k) { const int rc = blur_check(p, in, outs[k]); if (rc) return rc; }
+    VQ_REQUIRE(row_begin >= 0 && row_end <= p->iImageSizeY && row_begin <= row_end, "row range out of bounds");
+    PostDests d;
+    int rc = post_dests_check(ctx, in, outs, n_outs, outs[0].width, outs[0].height, "every destination must have the size of the first",
+                              "blur: in-place is not supported (the engine ping-pongs too)", row_begin, row_end, signal, d); if (rc) return rc;
+    rc = vq_enter(ctx); if (rc) return rc;
+    VQ_MARK("Blur");
+    if (row_begin == row_end) return VQ_OK;
+    const unsigned gy = post_tile_rows(ctx, d, B2_TH, 0, B2_TH - 1, (p->iImageSizeY + B2_TH - 1) / B2_TH);
+    return blur2d_launch<true>(dim3((p->iImageSizeX + B2_TW - 1) / B2_TW, gy), make_view(in), d, p->iImageSizeX, p->iImageSizeY,
+                               (cudaStream_t)stream);
 }
 
 extern "C" int vq_fsr_easu_source_rows(const uint32_t con[16], int address_mode, int in_height, int out_height, int row_begin,

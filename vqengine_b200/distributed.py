@@ -6,7 +6,8 @@ finished tiles at the end (NCCL over NVLink on the GPU box; gloo in the CPU test
 GPU, torch.distributed for the plumbing. Nothing here computes pixels.
 
 Row spaces:
-  forward / post passes : image rows                      -> equal contiguous row blocks (post chain halos: post_chain_rows)
+  forward / post passes : image rows                      -> equal contiguous row blocks (post chain halos: post_chain_rows,
+                                                             with the blur in front: blur_rows)
   diffuse irradiance    : face*res + row                  -> equal contiguous row blocks
   specular prefilter    : flattened (mip, face, row)      -> contiguous blocks of equal COST
                           (a row of mip m has (res>>m) texels; mip 0 is roughness 0 = ~1 % of a full texel,
@@ -60,6 +61,15 @@ def post_chain_rows(in_height: int, out_height: int, band: Tuple[int, int], fsr_
     if cas:
         return {"tonemap": [halo], "cas": [(a, b)]}
     return {"tonemap": [(a, b)]}
+
+
+def blur_rows(in_height: int, out_height: int, band: Tuple[int, int], fsr_con=None, address_mode: int = 0,
+              cas: bool = False) -> Dict[str, List[Tuple[int, int]]]:
+    """post_chain_rows with the Gaussian blur of the HDR frame in front of the chain: a "gaussian_blur" stage whose output rows are
+    the tonemapper's source rows (the band plus the halo EASU, RCAS or CAS read), which vq_gaussian_blur_multi_signal produces from
+    the whole source frame (it reads rows 10 beyond each range, clamped, itself). in_height is also the blur's iImageSizeY."""
+    plan = post_chain_rows(in_height, out_height, band, fsr_con, address_mode, cas)
+    return {"gaussian_blur": list(plan["tonemap"]), **plan}
 
 
 def weighted_tiles(costs: Sequence[float], world: int) -> List[Tuple[int, int]]:
