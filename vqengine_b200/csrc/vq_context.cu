@@ -58,6 +58,25 @@ int vq_fill_peer_sync(const VqContext* ctx, const VqPeerSignal* sig, PeerSync* o
     return VQ_OK;
 }
 
+// ---- the band contract (every *_multi_signal call) ----------------------------------------------------------------------------
+int vq_band_list(const void* outs, int n_outs) {
+    VQ_REQUIRE(outs, "null destination list");
+    VQ_REQUIRE(n_outs >= 1 && n_outs <= 8, "1..8 destinations");
+    return VQ_OK;
+}
+
+int vq_band_check(const VqContext* ctx, int n_outs, int dst_row_offset, int H, int row_begin, int row_end, const VqPeerSignal* sig,
+                  PeerSync& sync) {
+    VQ_REQUIRE(dst_row_offset >= 0, "negative destination row offset");
+    VQ_REQUIRE(row_begin >= 0 && row_end <= H && row_begin <= row_end, "row range out of bounds");
+    VQ_REQUIRE(row_begin < row_end || !(sig && sig->n_ranks > 1), "a rendezvous needs a non-empty row range (the kernel runs it)");
+    const int rc = vq_fill_peer_sync(ctx, sig, &sync); if (rc) return rc;
+    VQ_REQUIRE(sync.n == 0 || n_outs > 1, "a rendezvous only makes sense with peer destinations");
+    return VQ_OK;
+}
+
+uint32_t* vq_band_ticket(VqContext* ctx, const PeerSync& sync) { return sync.n > 1 ? vq_ticket_pair(ctx) : nullptr; }
+
 // vq_ctx_rendezvous_clear: the record and the cancel word zeroed in stream order (loaded when the first deadline is registered)
 __global__ void rendezvous_clear_kernel(VqRendezvousStatus* status, uint32_t* cancel) {
     *status = VqRendezvousStatus{};

@@ -1079,34 +1079,35 @@ static int frame_params(VqContext* ctx, const VqPerFrameData* pf, const VqPerVie
     return VQ_OK;
 }
 
-// The destinations, row range and rendezvous of a multi-destination call over a W x H source (G-buffer or attribute planes):
-// 1..8 frames as wide as the source that hold dst_row_offset + H rows, rows inside the source, a signal only with peer
-// destinations and rows to shade (its last CTA runs the rendezvous). Host-side only; fills `sync` from `sig`.
-int vq_multi_dest_check(const VqContext* ctx, const VqImage* outs, int n_outs, int W, int H, int dst_row_offset, int row_begin,
-                        int row_end, const VqPeerSignal* sig, PeerSync& sync) {
-    VQ_REQUIRE(n_outs >= 1 && n_outs <= 8, "1..8 destinations");
-    VQ_REQUIRE(dst_row_offset >= 0, "negative destination row offset");
+// The forward passes' band destinations over a W x H source (G-buffer or attribute planes): frames as wide as the source that
+// hold dst_row_offset + H rows, between the shared band checks. Fills `sync` from `sig`.
+static int forward_band_check(const VqContext* ctx, const VqImage* outs, int n_outs, int W, int H, int dst_row_offset, int row_begin,
+                              int row_end, const VqPeerSignal* sig, PeerSync& sync) {
+    int rc = vq_band_list(outs, n_outs); if (rc) return rc;
     for (int k = 0; k < n_outs; ++k)
         VQ_REQUIRE(vq_image_ok(outs[k]) && outs[k].width == W && outs[k].height >= dst_row_offset + H,
                    "every destination must be as wide as the G-buffer and hold dst_row_offset + height rows");
-    VQ_REQUIRE(row_begin >= 0 && row_end <= H && row_begin <= row_end, "row range out of bounds");
-    VQ_REQUIRE(row_begin < row_end || !(sig && sig->n_ranks > 1), "a rendezvous needs a non-empty row range (the kernel runs it)");
-    const int rc = vq_fill_peer_sync(ctx, sig, &sync); if (rc) return rc;
-    VQ_REQUIRE(sync.n == 0 || n_outs > 1, "a rendezvous only makes sense with peer destinations");
-    return VQ_OK;
+    return vq_band_check(ctx, n_outs, dst_row_offset, H, row_begin, row_end, sig, sync);
 }
 
-int vq_forward_launch_multi(VqContext* ctx, const VqPerFrameData* pf, const VqPerViewLightingData* pv,
-                            const VqGBuffer* gb, const VqEnvironmentMaps* env, const VqImage* outs, int n_outs,
-                            int dst_row_offset, int row_begin, int row_end, const VqPeerSignal* sig, cudaStream_t stream,
-                            const ShadowRecV* shadow) {
+int vq_forward_check(const VqContext* ctx, const VqPerFrameData* pf, const VqPerViewLightingData* pv, const VqGBuffer* gb,
+                     const VqEnvironmentMaps* env, const VqImage* outs, int n_outs, int dst_row_offset, int row_begin, int row_end,
+                     const VqPeerSignal* sig, PeerSync& sync) {
     VQ_REQUIRE(pf && pv && gb && env && outs, "null parameter block");
     VQ_REQUIRE(vq_image_ok(gb->position_ao) && vq_image_ok(gb->normal_roughness) && vq_image_ok(gb->albedo_metalness), "bad image descriptor");
     const int W = gb->position_ao.width, H = gb->position_ao.height;
     VQ_REQUIRE(gb->normal_roughness.width == W && gb->albedo_metalness.width == W &&
                gb->normal_roughness.height == H && gb->albedo_metalness.height == H, "G-buffer planes must have the same size");
-    PeerSync sync;
-    int rc = vq_multi_dest_check(ctx, outs, n_outs, W, H, dst_row_offset, row_begin, row_end, sig, sync); if (rc) return rc;
+    if (gb->emissive.ptr)
+        VQ_REQUIRE(vq_image_ok(gb->emissive) && gb->emissive.width == W && gb->emissive.height == H, "bad emissive plane");
+    return forward_band_check(ctx, outs, n_outs, W, H, dst_row_offset, row_begin, row_end, sig, sync);
+}
+
+int vq_forward_launch_multi(VqContext* ctx, const VqPerFrameData* pf, const VqPerViewLightingData* pv,
+                            const VqGBuffer* gb, const VqEnvironmentMaps* env, const VqImage* outs, int n_outs,
+                            int dst_row_offset, int row_begin, int row_end, const PeerSync& sync, cudaStream_t stream,
+                            const ShadowRecV* shadow) {
+    const int W = gb->position_ao.width;
     const VqSceneLighting& L = pf->Lights;
     VQ_REQUIRE(light_counts_ok(L), "light counts exceed the cbuffer arrays");
     if (row_begin == row_end) return VQ_OK;
@@ -1118,11 +1119,8 @@ int vq_forward_launch_multi(VqContext* ctx, const VqPerFrameData* pf, const VqPe
     for (int k = 0; k < n_outs; ++k) P.outs[k] = make_view(outs[k]);
     P.nOut = n_outs; P.dstRowOffset = dst_row_offset;
     P.hasEmissive = gb->emissive.ptr != nullptr;
-    if (P.hasEmissive) {
-        VQ_REQUIRE(vq_image_ok(gb->emissive) && gb->emissive.width == W && gb->emissive.height == H, "bad emissive plane");
-        P.emi = make_view(gb->emissive);
-    }
-    rc = frame_params(ctx, pf, pv, env, stream, P); if (rc) return rc;
+    if (P.hasEmissive) P.emi = make_view(gb->emissive);
+    int rc = frame_params(ctx, pf, pv, env, stream, P); if (rc) return rc;
     P.rowBegin = row_begin; P.rows = row_end - row_begin; P.width = W;
     const bool shadowed = shadow && shadow->p;
     if (shadowed) {
@@ -1130,9 +1128,7 @@ int vq_forward_launch_multi(VqContext* ctx, const VqPerFrameData* pf, const VqPe
                    "PCF records do not match the frame's caster lists");
         P.shadow = *shadow;
     }
-
     P.sync = sync;
-    P.ticket = P.sync.n > 1 ? vq_ticket_pair(ctx) : nullptr;
 
     // persistent grid: x = the row's 256-pixel tiles, y = row groups striding the rows
     const unsigned gx = (unsigned)((W + FWD_TILE - 1) / FWD_TILE);
@@ -1163,6 +1159,7 @@ int vq_forward_launch_multi(VqContext* ctx, const VqPerFrameData* pf, const VqPe
         return VQ_OK;
     };
     VQ_REQUIRE(smem <= 96 * 1024, "stage layout exceeds the shared-memory budget");
+    P.ticket = vq_band_ticket(ctx, P.sync);
     if (shadowed && n_outs > 1) rc = rot ? launch(forward_kernel<true, true, true>) : launch(forward_kernel<true, false, true>);
     else if (shadowed) rc = rot ? launch(forward_kernel<false, true, true>) : launch(forward_kernel<false, false, true>);
     else if (n_outs > 1) rc = rot ? launch(forward_kernel<true, true>) : launch(forward_kernel<true, false>);
@@ -1171,11 +1168,20 @@ int vq_forward_launch_multi(VqContext* ctx, const VqPerFrameData* pf, const VqPe
     return vq_check_launch("forward_lighting");
 }
 
+// the G-buffer pass without shadow maps: checked, then launched
+static int forward_call(VqContext* ctx, const VqPerFrameData* pf, const VqPerViewLightingData* pv, const VqGBuffer* gb,
+                        const VqEnvironmentMaps* env, const VqImage* outs, int n_outs, int dst_row_offset, int row_begin, int row_end,
+                        const VqPeerSignal* sig, cudaStream_t stream) {
+    PeerSync sync;
+    const int rc = vq_forward_check(ctx, pf, pv, gb, env, outs, n_outs, dst_row_offset, row_begin, row_end, sig, sync); if (rc) return rc;
+    return vq_forward_launch_multi(ctx, pf, pv, gb, env, outs, n_outs, dst_row_offset, row_begin, row_end, sync, stream);
+}
+
 int vq_forward_launch(VqContext* ctx, const VqPerFrameData* pf, const VqPerViewLightingData* pv,
                       const VqGBuffer* gb, const VqEnvironmentMaps* env, VqImage out,
-                      int row_begin, int row_end, cudaStream_t stream, const ShadowRecV* shadow) {
+                      int row_begin, int row_end, cudaStream_t stream) {
     VQ_REQUIRE(gb && vq_image_ok(out) && out.height == gb->position_ao.height, "G-buffer planes and output must have the same size");
-    return vq_forward_launch_multi(ctx, pf, pv, gb, env, &out, 1, 0, row_begin, row_end, nullptr, stream, shadow);
+    return forward_call(ctx, pf, pv, gb, env, &out, 1, 0, row_begin, row_end, nullptr, stream);
 }
 
 extern "C" int vq_forward_lighting(VqContext* ctx, const VqPerFrameData* pf, const VqPerViewLightingData* pv,
@@ -1189,9 +1195,7 @@ extern "C" int vq_forward_lighting(VqContext* ctx, const VqPerFrameData* pf, con
 extern "C" int vq_forward_lighting_multi(VqContext* ctx, const VqPerFrameData* pf, const VqPerViewLightingData* pv,
                                          const VqGBuffer* gb, const VqEnvironmentMaps* env, const VqImage* outs, int n_outs,
                                          int dst_row_offset, int row_begin, int row_end, void* stream) {
-    int rc = vq_enter(ctx); if (rc) return rc;
-    VQ_MARK("RenderSceneColor");
-    return vq_forward_launch_multi(ctx, pf, pv, gb, env, outs, n_outs, dst_row_offset, row_begin, row_end, nullptr, (cudaStream_t)stream);
+    return vq_forward_lighting_multi_signal(ctx, pf, pv, gb, env, outs, n_outs, dst_row_offset, row_begin, row_end, nullptr, stream);
 }
 
 // the same, with the cross-rank rendezvous run by the kernel's last CTA (VqPeerSignal): one kernel = shade + gather + barrier
@@ -1200,7 +1204,7 @@ extern "C" int vq_forward_lighting_multi_signal(VqContext* ctx, const VqPerFrame
                                                 int dst_row_offset, int row_begin, int row_end, const VqPeerSignal* signal, void* stream) {
     int rc = vq_enter(ctx); if (rc) return rc;
     VQ_MARK("RenderSceneColor");
-    return vq_forward_launch_multi(ctx, pf, pv, gb, env, outs, n_outs, dst_row_offset, row_begin, row_end, signal, (cudaStream_t)stream);
+    return forward_call(ctx, pf, pv, gb, env, outs, n_outs, dst_row_offset, row_begin, row_end, signal, (cudaStream_t)stream);
 }
 
 // PSMain from interpolants and materials in one launch (psmain_kernel): what vq_gbuffer_from_materials with an emissive plane
@@ -1218,7 +1222,7 @@ static int psmain_launch(VqContext* ctx, const VqPerFrameData* pf, const VqPerVi
     memset(&Q, 0, sizeof(Q));
     int rc;
     if (multi) {
-        rc = vq_multi_dest_check(ctx, outs, n_outs, W, H, dst_row_offset, row_begin, row_end, sig, Q.F.sync); if (rc) return rc;
+        rc = forward_band_check(ctx, outs, n_outs, W, H, dst_row_offset, row_begin, row_end, sig, Q.F.sync); if (rc) return rc;
         // the surface producer's quads sit on even rows of the attribute planes: an even offset keeps them on even rows of the frame
         VQ_REQUIRE((dst_row_offset & 1) == 0, "dst_row_offset must be even (quads are aligned to even rows)");
     } else {
@@ -1241,7 +1245,7 @@ static int psmain_launch(VqContext* ctx, const VqPerFrameData* pf, const VqPerVi
     P.hasEmissive = 1;
     for (int k = 0; k < n_outs; ++k) P.outs[k] = make_view(outs[k]);
     P.nOut = n_outs; P.dstRowOffset = dst_row_offset;
-    P.ticket = P.sync.n > 1 ? vq_ticket_pair(ctx) : nullptr;
+    P.ticket = vq_band_ticket(ctx, P.sync);
     P.rowBegin = row_begin; P.rows = row_end - row_begin; P.width = W;
     // persistent grid: x = the row's 128-column tiles, y = groups striding the row pairs
     const unsigned gx = (unsigned)((W + FWD_THREADS - 1) / FWD_THREADS);

@@ -46,11 +46,11 @@ constexpr int IBL_THREADS = 256;
 constexpr int IBL_WARPS = IBL_THREADS / 32;
 
 struct DiffuseArgs {
-    PyrV hdri; float4* out; int res; int rowBegin; int texels;   // texels = rows * res
+    PyrV hdri; int res; int rowBegin; int texels;   // texels = rows * res
     float step; int nPhi, nTheta; int srcMip;
 };
-// The multi-destination form (vq_diffuse_irradiance_multi_signal): every texel goes to each of n packed cubemaps (the local one
-// first, then the peers'), and the last CTA to retire runs the rendezvous (cta_retire). A.out is unused.
+// Every texel goes to each of n packed cubemaps (the local one first, then the peers'), and with a rendezvous the last CTA to retire
+// runs it (cta_retire). vq_diffuse_irradiance is the band form with one destination and no rendezvous.
 struct DiffuseMultiArgs {
     DiffuseArgs a;
     float4* o[8]; int n;
@@ -109,11 +109,6 @@ __device__ __forceinline__ void diffuse_texels(const DiffuseArgs& A, float* smem
             store((size_t)fr * A.res + px, make_float4(PI * acc.x / n, PI * acc.y / n, PI * acc.z / n, 1.0f));
         }
     }
-}
-
-__global__ void __launch_bounds__(IBL_THREADS) diffuse_irradiance_kernel(const __grid_constant__ DiffuseArgs A) {
-    extern __shared__ float smem[];
-    diffuse_texels(A, smem, [&](size_t i, float4 o) { A.out[i] = o; });
 }
 
 __global__ void __launch_bounds__(IBL_THREADS) diffuse_irradiance_multi_kernel(const __grid_constant__ DiffuseMultiArgs M) {
@@ -380,15 +375,24 @@ extern "C" int vq_hdri_build_mips(VqContext* ctx, VqPyramid hd, void* stream) {
     return VQ_OK;
 }
 
-// K2's argument checks and launch parameters (every field of A but A.out), shared by the single and the multi-destination call
-static int diffuse_setup(const VqDiffuseIrradianceParams* p, VqPyramid hd, VqCubemap out, int row_begin, int row_end,
-                         DiffuseArgs& A, size_t& smem) {
+// K2 on rows [row_begin, row_end) into every destination cubemap, with the optional in-kernel rendezvous: the band call, and the
+// single call with one destination and no signal. Every argument is checked before the device is touched.
+static int diffuse_launch(VqContext* ctx, const VqDiffuseIrradianceParams* p, VqPyramid hd, const VqCubemap* outs, int n_outs,
+                          int row_begin, int row_end, const VqPeerSignal* sig, cudaStream_t stream, const char* what) {
+    int rc = vq_band_list(outs, n_outs); if (rc) return rc;
     VQ_REQUIRE(p, "params is null");
     VQ_REQUIRE(pyr_ok(hd), "bad HDRI pyramid descriptor");
+    const VqCubemap out = outs[0];
     VQ_REQUIRE(out.ptr && out.res >= 2 && out.mips == 1, "diffuse irradiance cubemap must have 1 mip");
     VQ_REQUIRE((out.res & 1) == 0, "cubemap resolution must be even (pole texel, SURVEY.md A32)");
     VQ_REQUIRE(p->src_mip >= 0 && p->src_mip < hd.levels, "src_mip outside the pyramid");
-    VQ_REQUIRE(row_begin >= 0 && row_end <= 6 * out.res && row_begin <= row_end, "row range out of bounds");
+    for (int k = 1; k < n_outs; ++k) {
+        VQ_REQUIRE(outs[k].ptr && outs[k].res == outs[0].res && outs[k].mips == outs[0].mips, "every destination cubemap must have the same shape");
+        VQ_REQUIRE(outs[k].ptr != outs[0].ptr, "a peer destination must not be the local cubemap outs[0]");
+    }
+    DiffuseMultiArgs M;
+    memset(&M, 0, sizeof(M));
+    rc = vq_band_check(ctx, n_outs, 0, 6 * out.res, row_begin, row_end, sig, M.sync); if (rc) return rc;
     int nPhi, nTheta;
     if (p->step > 0.0f) {
         // trip counts of the float-accumulated loops (CubemapConvolution.hlsl:129,133)
@@ -396,62 +400,36 @@ static int diffuse_setup(const VqDiffuseIrradianceParams* p, VqPyramid hd, VqCub
         nTheta = 0; for (float th = 0.0f; th < 1.5707963268f; th += p->step) { if (++nTheta > (1 << 20)) break; }
     } else { nPhi = p->n_phi; nTheta = p->n_theta; }
     VQ_REQUIRE(nPhi >= 1 && nTheta >= 1 && (long long)nPhi * nTheta < (1 << 24), "sample grid out of range");
-    smem = (size_t)(2 * nPhi + 2 * nTheta) * sizeof(float);
+    const size_t smem = (size_t)(2 * nPhi + 2 * nTheta) * sizeof(float);
     VQ_REQUIRE(smem <= 200 * 1024, "sample grid does not fit shared memory");
-    A.hdri = make_pyr(hd); A.out = nullptr; A.res = out.res; A.rowBegin = row_begin;
+    DiffuseArgs& A = M.a;
+    A.hdri = make_pyr(hd); A.res = out.res; A.rowBegin = row_begin;
     A.texels = (row_end - row_begin) * out.res;
     A.step = p->step > 0.0f ? p->step : 0.0f; A.nPhi = nPhi; A.nTheta = nTheta; A.srcMip = p->src_mip;
-    return VQ_OK;
-}
-
-// K2's grid: one warp per texel, at most 8 CTAs per SM (the CTAs stride over the texels)
-static int diffuse_blocks(const VqContext* ctx, int texels) {
-    int blocks = (texels + IBL_WARPS - 1) / IBL_WARPS;
-    const int cap = ctx->sm_count * 8;
-    return blocks > cap ? cap : blocks;
+    for (int k = 0; k < n_outs; ++k) M.o[k] = (float4*)outs[k].ptr;
+    M.n = n_outs;
+    rc = vq_enter(ctx); if (rc) return rc;
+    VQ_MARK("DiffuseIrradianceCubemap");
+    if (row_begin == row_end) return VQ_OK;
+    M.ticket = vq_band_ticket(ctx, M.sync);
+    if (smem > 48 * 1024) VQ_CUDA_OK(cudaFuncSetAttribute(diffuse_irradiance_multi_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    int blocks = (M.a.texels + IBL_WARPS - 1) / IBL_WARPS;         // one warp per texel, at most 8 CTAs per SM (striding the texels)
+    if (blocks > ctx->sm_count * 8) blocks = ctx->sm_count * 8;
+    diffuse_irradiance_multi_kernel<<<blocks, IBL_THREADS, smem, stream>>>(M);
+    return vq_check_launch(what);
 }
 
 extern "C" int vq_diffuse_irradiance(VqContext* ctx, const VqDiffuseIrradianceParams* p, VqPyramid hd, VqCubemap out,
                                      int row_begin, int row_end, void* stream) {
-    int rc = vq_enter(ctx); if (rc) return rc;
-    VQ_MARK("DiffuseIrradianceCubemap");
-    DiffuseArgs A;
-    size_t smem = 0;
-    rc = diffuse_setup(p, hd, out, row_begin, row_end, A, smem); if (rc) return rc;
-    if (row_begin == row_end) return VQ_OK;
-    A.out = (float4*)out.ptr;
-    if (smem > 48 * 1024) VQ_CUDA_OK(cudaFuncSetAttribute(diffuse_irradiance_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    diffuse_irradiance_kernel<<<diffuse_blocks(ctx, A.texels), IBL_THREADS, smem, (cudaStream_t)stream>>>(A);
-    return vq_check_launch("diffuse_irradiance");
+    const int rc = vq_enter(ctx); if (rc) return rc;               // the single call refuses a null context first
+    return diffuse_launch(ctx, p, hd, &out, 1, row_begin, row_end, nullptr, (cudaStream_t)stream, "diffuse_irradiance");
 }
 
-// K2 on rows [row_begin, row_end) into every destination cubemap (one rank's band of a multi-GPU prefilter), with the optional
-// in-kernel rendezvous. Every argument is checked before the device is touched.
+// one rank's band of a multi-GPU prefilter
 extern "C" int vq_diffuse_irradiance_multi_signal(VqContext* ctx, const VqDiffuseIrradianceParams* p, VqPyramid hd,
                                                   const VqCubemap* outs, int n_outs, int row_begin, int row_end,
                                                   const VqPeerSignal* signal, void* stream) {
-    VQ_REQUIRE(outs, "null destination list");
-    VQ_REQUIRE(n_outs >= 1 && n_outs <= 8, "1..8 destinations");
-    DiffuseMultiArgs M;
-    memset(&M, 0, sizeof(M));
-    size_t smem = 0;
-    int rc = diffuse_setup(p, hd, outs[0], row_begin, row_end, M.a, smem); if (rc) return rc;
-    for (int k = 1; k < n_outs; ++k) {
-        VQ_REQUIRE(outs[k].ptr && outs[k].res == outs[0].res && outs[k].mips == outs[0].mips, "every destination cubemap must have the same shape");
-        VQ_REQUIRE(outs[k].ptr != outs[0].ptr, "a peer destination must not be the local cubemap outs[0]");
-    }
-    VQ_REQUIRE(row_begin < row_end || !(signal && signal->n_ranks > 1), "a rendezvous needs a non-empty row range (the kernel runs it)");
-    rc = vq_fill_peer_sync(ctx, signal, &M.sync); if (rc) return rc;
-    VQ_REQUIRE(M.sync.n == 0 || n_outs > 1, "a rendezvous only makes sense with peer destinations");
-    rc = vq_enter(ctx); if (rc) return rc;
-    VQ_MARK("DiffuseIrradianceCubemap");
-    if (row_begin == row_end) return VQ_OK;
-    for (int k = 0; k < n_outs; ++k) M.o[k] = (float4*)outs[k].ptr;
-    M.n = n_outs;
-    M.ticket = M.sync.n > 1 ? vq_ticket_pair(ctx) : nullptr;
-    if (smem > 48 * 1024) VQ_CUDA_OK(cudaFuncSetAttribute(diffuse_irradiance_multi_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    diffuse_irradiance_multi_kernel<<<diffuse_blocks(ctx, M.a.texels), IBL_THREADS, smem, (cudaStream_t)stream>>>(M);
-    return vq_check_launch("diffuse_irradiance_multi");
+    return diffuse_launch(ctx, p, hd, outs, n_outs, row_begin, row_end, signal, (cudaStream_t)stream, "diffuse_irradiance_multi");
 }
 
 // ranges: n_ranges pairs [begin,end) of the flattened (mip, face, row) space, in increasing order and disjoint
@@ -566,27 +544,23 @@ extern "C" int vq_brdf_integration_lut(VqContext* ctx, VqImage out, int num_samp
 // argument is checked before the device is touched.
 extern "C" int vq_brdf_integration_lut_multi_signal(VqContext* ctx, const VqImage* outs, int n_outs, int num_samples, int row_begin,
                                                     int row_end, const VqPeerSignal* signal, void* stream) {
-    VQ_REQUIRE(outs, "null destination list");
-    VQ_REQUIRE(n_outs >= 1 && n_outs <= 8, "1..8 destinations");
+    int rc = vq_band_list(outs, n_outs); if (rc) return rc;
     for (int k = 0; k < n_outs; ++k) {
         VQ_REQUIRE(vq_image_ok(outs[k], 8), "bad LUT image descriptor (float2 texels)");
         VQ_REQUIRE(outs[k].width == outs[0].width && outs[k].height == outs[0].height, "every destination must have the size of the first");
         VQ_REQUIRE(k == 0 || outs[k].ptr != outs[0].ptr, "a peer destination must not be the local LUT outs[0]");
     }
     VQ_REQUIRE(num_samples >= 1 && num_samples <= 8192, "num_samples out of range");
-    VQ_REQUIRE(row_begin >= 0 && row_end <= outs[0].height && row_begin <= row_end, "row range out of bounds");
-    VQ_REQUIRE(row_begin < row_end || !(signal && signal->n_ranks > 1), "a rendezvous needs a non-empty row range (the kernel runs it)");
     LutMultiArgs M;
     memset(&M, 0, sizeof(M));
-    int rc = vq_fill_peer_sync(ctx, signal, &M.sync); if (rc) return rc;
-    VQ_REQUIRE(M.sync.n == 0 || n_outs > 1, "a rendezvous only makes sense with peer destinations");
+    rc = vq_band_check(ctx, n_outs, 0, outs[0].height, row_begin, row_end, signal, M.sync); if (rc) return rc;
     rc = vq_enter(ctx); if (rc) return rc;
     VQ_MARK("CreateBRDFIntegralLUT");
     if (row_begin == row_end) return VQ_OK;
     M.a.w = outs[0].width; M.a.h = outs[0].height; M.a.rowBegin = row_begin; M.a.numSamples = num_samples;
     for (int k = 0; k < n_outs; ++k) { M.o[k] = (float2*)outs[k].ptr; M.pitch2[k] = (int)(outs[k].pitch_bytes / 8); }
     M.n = n_outs;
-    M.ticket = M.sync.n > 1 ? vq_ticket_pair(ctx) : nullptr;
+    M.ticket = vq_band_ticket(ctx, M.sync);
     const size_t smem = (size_t)num_samples * sizeof(float4);
     if (smem > 48 * 1024) VQ_CUDA_OK(cudaFuncSetAttribute(brdf_lut_multi_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     const dim3 grid((outs[0].width + 255) / 256, row_end - row_begin);

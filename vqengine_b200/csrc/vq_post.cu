@@ -992,23 +992,26 @@ extern "C" int vq_fsr_easu(VqContext* ctx, const uint32_t con[16], int address_m
 // =============================================================================================
 // K6-K9 on a band of the output into several frames (vq_*_multi_signal): one rank's share of the post chain
 // =============================================================================================
-// The destination checks every multi-destination post call shares, before the device is touched: 1..8 destinations of exactly the
-// W x H output (`size_msg`, the single call's message, otherwise), none equal to `in` unless the pass may run in place
-// (`alias_msg` == nullptr: the tonemapper), then the row range and the signal as vq_multi_dest_check takes them. Fills `d`.
+// vq_band_check over `rows` output rows once a post call's own destination checks have passed. Fills `d`.
+static int post_band(const VqContext* ctx, const VqImage* outs, int n_outs, int rows, int row_begin, int row_end, const VqPeerSignal* sig,
+                     PostDests& d) {
+    memset(&d, 0, sizeof(d));
+    const int rc = vq_band_check(ctx, n_outs, 0, rows, row_begin, row_end, sig, d.sync); if (rc) return rc;
+    for (int k = 0; k < n_outs; ++k) d.o[k] = make_view(outs[k]);
+    d.n = n_outs; d.w = outs[0].width; d.h = outs[0].height; d.rowBegin = row_begin; d.rowEnd = row_end;
+    return VQ_OK;
+}
+
+// A post band call's destinations after vq_band_list: frames of exactly the W x H output (`size_msg`, the single call's message,
+// otherwise), none equal to `in` unless the pass may run in place (`alias_msg` == nullptr: the tonemapper); then post_band.
 static int post_dests_check(const VqContext* ctx, VqImage in, const VqImage* outs, int n_outs, int W, int H, const char* size_msg, const char* alias_msg,
                             int row_begin, int row_end, const VqPeerSignal* sig, PostDests& d) {
-    VQ_REQUIRE(outs, "null destination list");
-    VQ_REQUIRE(n_outs >= 1 && n_outs <= 8, "1..8 destinations");
     for (int k = 0; k < n_outs; ++k) {
         VQ_REQUIRE(vq_image_ok(outs[k]), "bad image descriptor");
         VQ_REQUIRE(outs[k].width == W && outs[k].height == H, size_msg);
         VQ_REQUIRE(!alias_msg || outs[k].ptr != in.ptr, alias_msg);
     }
-    memset(&d, 0, sizeof(d));
-    const int rc = vq_multi_dest_check(ctx, outs, n_outs, W, H, 0, row_begin, row_end, sig, d.sync); if (rc) return rc;
-    for (int k = 0; k < n_outs; ++k) d.o[k] = make_view(outs[k]);
-    d.n = n_outs; d.w = W; d.h = H; d.rowBegin = row_begin; d.rowEnd = row_end;
-    return VQ_OK;
+    return post_band(ctx, outs, n_outs, H, row_begin, row_end, sig, d);
 }
 
 static int floor_div(int a, int b) { return a >= 0 ? a / b : -((-a + b - 1) / b); }
@@ -1019,7 +1022,7 @@ static unsigned post_tile_rows(VqContext* ctx, PostDests& d, int tile, int lo, i
     const int first = std::max(0, floor_div(d.rowBegin - hi + tile - 1, tile));
     const int last = std::min(n_tiles - 1, floor_div(d.rowEnd - 1 - lo, tile));
     d.by0 = first;
-    d.ticket = d.sync.n > 1 ? vq_ticket_pair(ctx) : nullptr;
+    d.ticket = vq_band_ticket(ctx, d.sync);
     return (unsigned)(last - first + 1);
 }
 
@@ -1027,8 +1030,9 @@ extern "C" int vq_tonemap_multi_signal(VqContext* ctx, const VqTonemapperParams*
                                        int row_begin, int row_end, const VqPeerSignal* signal, void* stream) {
     VQ_REQUIRE(p, "params is null");
     VQ_REQUIRE(vq_image_ok(in), "bad image descriptor");
+    int rc = vq_band_list(outs, n_outs); if (rc) return rc;
     PostDests d;
-    int rc = post_dests_check(ctx, in, outs, n_outs, in.width, in.height, "tonemap: in/out size mismatch", nullptr, row_begin, row_end,
+    rc = post_dests_check(ctx, in, outs, n_outs, in.width, in.height, "tonemap: in/out size mismatch", nullptr, row_begin, row_end,
                               signal, d); if (rc) return rc;
     rc = vq_enter(ctx); if (rc) return rc;
     VQ_MARK("TonemapperCS");
@@ -1042,8 +1046,9 @@ extern "C" int vq_cas_multi_signal(VqContext* ctx, const uint32_t cas_const[8], 
                                    int row_begin, int row_end, const VqPeerSignal* signal, void* stream) {
     VQ_REQUIRE(cas_const, "cas_const is null");
     VQ_REQUIRE(vq_image_ok(in), "bad image descriptor");
+    int rc = vq_band_list(outs, n_outs); if (rc) return rc;
     PostDests d;
-    int rc = post_dests_check(ctx, in, outs, n_outs, in.width, in.height, "cas: sharpen-only path needs equal sizes (FFXCAS_NO_UPSCALING)",
+    rc = post_dests_check(ctx, in, outs, n_outs, in.width, in.height, "cas: sharpen-only path needs equal sizes (FFXCAS_NO_UPSCALING)",
                               "cas: in-place is not supported", row_begin, row_end, signal, d); if (rc) return rc;
     rc = vq_enter(ctx); if (rc) return rc;
     VQ_MARK("FFX-CAS CS");
@@ -1058,8 +1063,9 @@ extern "C" int vq_fsr_rcas_multi_signal(VqContext* ctx, const uint32_t rcas_cons
                                         int row_begin, int row_end, const VqPeerSignal* signal, void* stream) {
     VQ_REQUIRE(rcas_const, "rcas_const is null");
     VQ_REQUIRE(vq_image_ok(in), "bad image descriptor");
+    int rc = vq_band_list(outs, n_outs); if (rc) return rc;
     PostDests d;
-    int rc = post_dests_check(ctx, in, outs, n_outs, in.width, in.height, "rcas: in/out size mismatch", "rcas: in-place is not supported",
+    rc = post_dests_check(ctx, in, outs, n_outs, in.width, in.height, "rcas: in/out size mismatch", "rcas: in-place is not supported",
                               row_begin, row_end, signal, d); if (rc) return rc;
     rc = vq_enter(ctx); if (rc) return rc;
     VQ_MARK("FSR-RCAS CS");
@@ -1075,9 +1081,10 @@ extern "C" int vq_fsr_easu_multi_signal(VqContext* ctx, const uint32_t con[16], 
     VQ_REQUIRE(con, "easu_const is null");
     VQ_REQUIRE(vq_image_ok(in), "bad image descriptor");
     VQ_REQUIRE(address_mode == VQ_ADDRESS_WRAP || address_mode == VQ_ADDRESS_CLAMP, "easu: unknown address mode");
-    const int W = outs && n_outs >= 1 ? outs[0].width : 0, H = outs && n_outs >= 1 ? outs[0].height : 0;
+    int rc = vq_band_list(outs, n_outs); if (rc) return rc;
+    const int W = outs[0].width, H = outs[0].height;
     PostDests d;
-    int rc = post_dests_check(ctx, in, outs, n_outs, W, H, "every destination must have the size of the first",
+    rc = post_dests_check(ctx, in, outs, n_outs, W, H, "every destination must have the size of the first",
                               "easu: in-place is not supported", row_begin, row_end, signal, d); if (rc) return rc;
     EasuCon c; memcpy(&c, con, 16);
     const float c0[4] = {c.c0x, c.c0y, c.c0z, c.c0w};
@@ -1114,13 +1121,13 @@ extern "C" int vq_fsr_easu_multi_signal(VqContext* ctx, const uint32_t con[16], 
 
 extern "C" int vq_gaussian_blur_multi_signal(VqContext* ctx, const VqBlurParams* p, VqImage in, const VqImage* outs, int n_outs,
                                              int row_begin, int row_end, const VqPeerSignal* signal, void* stream) {
-    VQ_REQUIRE(outs, "null destination list");
-    VQ_REQUIRE(n_outs >= 1 && n_outs <= 8, "1..8 destinations");
-    for (int k = 0; k < n_outs; ++k) { const int rc = blur_check(p, in, outs[k]); if (rc) return rc; }
-    VQ_REQUIRE(row_begin >= 0 && row_end <= p->iImageSizeY && row_begin <= row_end, "row range out of bounds");
+    int rc = vq_band_list(outs, n_outs); if (rc) return rc;
+    for (int k = 0; k < n_outs; ++k) {
+        rc = blur_check(p, in, outs[k]); if (rc) return rc;
+        VQ_REQUIRE(outs[k].width == outs[0].width && outs[k].height == outs[0].height, "every destination must have the size of the first");
+    }
     PostDests d;
-    int rc = post_dests_check(ctx, in, outs, n_outs, outs[0].width, outs[0].height, "every destination must have the size of the first",
-                              "blur: in-place is not supported (the engine ping-pongs too)", row_begin, row_end, signal, d); if (rc) return rc;
+    rc = post_band(ctx, outs, n_outs, p->iImageSizeY, row_begin, row_end, signal, d); if (rc) return rc;
     rc = vq_enter(ctx); if (rc) return rc;
     VQ_MARK("Blur");
     if (row_begin == row_end) return VQ_OK;
@@ -1412,11 +1419,10 @@ extern "C" int vq_post_process_multi_signal(VqContext* ctx, const VqTonemapperPa
                                             const uint32_t easu_const[16], int address_mode, const uint32_t rcas_const[4],
                                             VqImage scene_color, const VqImage* outs, int n_outs, int row_begin, int row_end,
                                             const VqPeerSignal* signal, void* stream) {
-    VQ_REQUIRE(outs, "null destination list");
-    VQ_REQUIRE(n_outs >= 1 && n_outs <= 8, "1..8 destinations");
+    int rc = vq_band_list(outs, n_outs); if (rc) return rc;
     const int W = outs[0].width, H = outs[0].height;
     PostPlan plan;
-    int rc = post_process_check(tonemapper, cas_const, easu_const, address_mode, rcas_const, scene_color, W, H, plan); if (rc) return rc;
+    rc = post_process_check(tonemapper, cas_const, easu_const, address_mode, rcas_const, scene_color, W, H, plan); if (rc) return rc;
     PostDests d;
     rc = post_dests_check(ctx, scene_color, outs, n_outs, W, H, "every destination must have the size of the first",
                           plan.fsr || plan.cas ? "post_process: in-place is not supported with EASU/RCAS or CAS" : nullptr,

@@ -149,18 +149,15 @@ bool vq_shadow_slots(const VqSceneLighting& L, const VqShadowMaps& sm, vq::Shado
 }
 
 // The PCF kernel over rows [row_begin, row_end) of the G-buffer, then the shadowed forward pass into outs[0..n_outs) (rows offset by
-// dst_row_offset, optional rendezvous); when no test runs, the plain forward pass. The shadow maps have been checked.
+// dst_row_offset, optional rendezvous); when no test runs, the plain forward pass. vq_forward_check and the shadow maps' checks
+// have passed.
 static int shadowed_passes(VqContext* ctx, const VqPerFrameData* pf, const VqPerViewLightingData* pv, const VqGBuffer* gb,
                            const VqEnvironmentMaps* env, const VqShadowMaps& sm, const VqImage* outs, int n_outs, int dst_row_offset,
-                           int row_begin, int row_end, const VqPeerSignal* sig, cudaStream_t stream) {
+                           int row_begin, int row_end, const PeerSync& sync, cudaStream_t stream) {
     vq::ShadowRecV V;
     const bool anyTest = vq_shadow_slots(pf->Lights, sm, V);
     if (!anyTest || row_begin >= row_end)          // no test runs: every factor is 1, which is what the plain kernel computes
-        return vq_forward_launch_multi(ctx, pf, pv, gb, env, outs, n_outs, dst_row_offset, row_begin, row_end, sig, stream);
-    VQ_REQUIRE(gb->position_ao.ptr && vq_image_ok(gb->position_ao) && vq_image_ok(gb->normal_roughness) &&
-               gb->normal_roughness.width == gb->position_ao.width && gb->normal_roughness.height == gb->position_ao.height,
-               "bad G-buffer planes");
-    VQ_REQUIRE(row_begin >= 0 && row_end <= gb->position_ao.height, "row range out of bounds");
+        return vq_forward_launch_multi(ctx, pf, pv, gb, env, outs, n_outs, dst_row_offset, row_begin, row_end, sync, stream);
 
     PcfParams P;
     memset(&P, 0, sizeof(P));
@@ -180,39 +177,30 @@ static int shadowed_passes(VqContext* ctx, const VqPerFrameData* pf, const VqPer
     rc = vq_check_launch("shadow_pcf"); if (rc) return rc;
 
     V.p = P.rec; V.pitch = P.recPitch;
-    return vq_forward_launch_multi(ctx, pf, pv, gb, env, outs, n_outs, dst_row_offset, row_begin, row_end, sig, stream, &V);
+    return vq_forward_launch_multi(ctx, pf, pv, gb, env, outs, n_outs, dst_row_offset, row_begin, row_end, sync, stream, &V);
 }
 
 extern "C" int vq_forward_lighting_shadowed(VqContext* ctx, const VqPerFrameData* pf, const VqPerViewLightingData* pv,
                                             const VqGBuffer* gb, const VqEnvironmentMaps* env, const VqShadowMaps* sm,
                                             VqImage out, int row_begin, int row_end, void* stream) {
-    int rc = vq_enter(ctx); if (rc) return rc;
-    VQ_MARK("RenderSceneColor");
-    VQ_REQUIRE(pf && pv && gb && env && sm, "null parameter block");
-    rc = vq_shadow_maps_check(pf->Lights, *sm); if (rc) return rc;
-    VQ_REQUIRE(vq_image_ok(out) && out.height == gb->position_ao.height, "G-buffer planes and output must have the same size");
-    return shadowed_passes(ctx, pf, pv, gb, env, *sm, &out, 1, 0, row_begin, row_end, nullptr, (cudaStream_t)stream);
+    const int rc = vq_enter(ctx); if (rc) return rc;               // the single call refuses a null context first
+    VQ_REQUIRE(gb && vq_image_ok(out) && out.height == gb->position_ao.height, "G-buffer planes and output must have the same size");
+    return vq_forward_lighting_shadowed_multi_signal(ctx, pf, pv, gb, env, sm, &out, 1, 0, row_begin, row_end, nullptr, stream);
 }
 
-// The same into n_outs frames (vq_forward_lighting_multi_signal's destinations, row offset and rendezvous). The shadow maps, the
-// G-buffer, the destinations, the row range and the signal are checked before the device is touched.
+// The same into n_outs frames (vq_forward_lighting_multi_signal's destinations, row offset and rendezvous). The G-buffer, the
+// destinations, the row range, the signal and the shadow maps are checked before the device is touched.
 extern "C" int vq_forward_lighting_shadowed_multi_signal(VqContext* ctx, const VqPerFrameData* pf, const VqPerViewLightingData* pv,
                                                          const VqGBuffer* gb, const VqEnvironmentMaps* env, const VqShadowMaps* sm,
                                                          const VqImage* outs, int n_outs, int dst_row_offset, int row_begin, int row_end,
                                                          const VqPeerSignal* signal, void* stream) {
-    VQ_REQUIRE(pf && pv && gb && env && sm && outs, "null parameter block");
-    int rc = vq_shadow_maps_check(pf->Lights, *sm); if (rc) return rc;
-    VQ_REQUIRE(vq_image_ok(gb->position_ao) && vq_image_ok(gb->normal_roughness) && vq_image_ok(gb->albedo_metalness), "bad image descriptor");
-    const int W = gb->position_ao.width, H = gb->position_ao.height;
-    VQ_REQUIRE(gb->normal_roughness.width == W && gb->albedo_metalness.width == W &&
-               gb->normal_roughness.height == H && gb->albedo_metalness.height == H, "G-buffer planes must have the same size");
-    if (gb->emissive.ptr)
-        VQ_REQUIRE(vq_image_ok(gb->emissive) && gb->emissive.width == W && gb->emissive.height == H, "bad emissive plane");
     PeerSync sync;
-    rc = vq_multi_dest_check(ctx, outs, n_outs, W, H, dst_row_offset, row_begin, row_end, signal, sync); if (rc) return rc;
+    int rc = vq_forward_check(ctx, pf, pv, gb, env, outs, n_outs, dst_row_offset, row_begin, row_end, signal, sync); if (rc) return rc;
+    VQ_REQUIRE(sm, "null parameter block");
+    rc = vq_shadow_maps_check(pf->Lights, *sm); if (rc) return rc;
     rc = vq_enter(ctx); if (rc) return rc;
     VQ_MARK("RenderSceneColor");
-    return shadowed_passes(ctx, pf, pv, gb, env, *sm, outs, n_outs, dst_row_offset, row_begin, row_end, signal, (cudaStream_t)stream);
+    return shadowed_passes(ctx, pf, pv, gb, env, *sm, outs, n_outs, dst_row_offset, row_begin, row_end, sync, (cudaStream_t)stream);
 }
 
 extern "C" int vq_depth_pyramid_level_count(int width, int height) { return vqshadow::depth_level_count(width, height); }
